@@ -81,8 +81,8 @@ int smcb_wmean_and_var(smcb_ctx *ctx, const double *W, const double *x, int64_t 
                                  u_in = N - 1 uniforms; synchronises once (ValueError check) */
 
 /* Inclusive prefix sum of non-negative fp64 values (the CDF that inverse_cdf,
- * resampling.py:484-509, walks).  Single pass, decoupled look-back with a
- * fixed association order: deterministic and non-decreasing by construction. */
+ * resampling.py:484-509, walks).  Reduce-then-scan with a fixed association
+ * order: deterministic and non-decreasing by construction. */
 int smcb_cumsum(smcb_ctx *ctx, const double *w, int64_t n, double *cdf_out);
 
 /* A[k] = min{ j : cdf[j] >= su[k] } clipped to n-1, for sorted su;
@@ -282,14 +282,6 @@ int smcb_filter_step_timed(smcb_filter *f, int64_t nsteps, double *out8);
  * out[0]=t, [1]=cur buffer index, [2]=rs_flag of last step, [3]=logLt, [4]=ESS,
  * [5]=log_mean_w, [6]=max lw, [7]=sum w */
 int smcb_filter_state(smcb_filter *f, double *out8);
-
-/* ---------------------------------------------------------------------------
- * measured ceilings of this device (bench.py "roofline.secondary"; no reference counterpart)
- * ------------------------------------------------------------------------- */
-/* fp64 FMA issue peak: out3 = {TFLOP/s, DFMA warp-instructions / cycle / SM at sm_mhz (0: skip), ms} */
-int smcb_measure_fp64_peak(smcb_ctx *ctx, double sm_mhz, double *out3_host);
-/* read + write streaming probe with 16-byte accesses over n doubles (n even): out1 = {GB/s} */
-int smcb_measure_stream_peak(smcb_ctx *ctx, const double *in, double *out, int64_t n, double *out1_host);
 
 #ifdef __cplusplus
 }

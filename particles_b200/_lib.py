@@ -93,8 +93,6 @@ PROTOTYPES = {
     "smcb_p2p_free": (C.c_int, [C.c_void_p]),
     "smcb_filter_step_timed": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_double)]),
     "smcb_filter_state": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),
-    "smcb_measure_fp64_peak": (C.c_int, [C.c_void_p, C.c_double, C.POINTER(C.c_double)]),
-    "smcb_measure_stream_peak": (C.c_int, [C.c_void_p, c_dp, c_dp, C.c_int64, C.POINTER(C.c_double)]),
 }
 
 _lib = None

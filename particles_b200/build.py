@@ -14,8 +14,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libsmcb.so")
-SOURCES = ["smcb_api.cu", "smcb_filter.cu", "smcb_filter_1d.cu", "smcb_filter_nd.cu", "smcb_sampler.cu",
-           "smcb_peaks.cu"]
+SOURCES = ["smcb_api.cu", "smcb_filter.cu", "smcb_filter_1d.cu", "smcb_filter_nd.cu", "smcb_sampler.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)
 NVCC_FLAGS = GENCODE + [
     "-O3", "-lineinfo", "-std=c++17",
@@ -62,7 +61,7 @@ def needs_build():
 
 
 def build(force=False, verbose=False, extra=None, out=None):
-    """``extra`` (or env SMCB_NVCC_EXTRA, space separated) appends compile flags, e.g. "-DSMCB_TABLE_MATH=1";
+    """``extra`` (or env SMCB_NVCC_EXTRA, space separated) appends compile flags, e.g. "-DSMCB_SPECULATE=0";
     ``out`` (or env SMCB_BUILD_OUT) names the library to write -- a FULL kernel-variant build next to the
     default one (select it with SMCB_LIB=<out>); the default library is untouched."""
     extra = extra if extra is not None else os.environ.get("SMCB_NVCC_EXTRA", "").split()

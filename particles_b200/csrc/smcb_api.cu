@@ -434,23 +434,14 @@ struct LoadResidual {
     }
 };
 
-template <typename T, typename LOAD>
-__global__ void __launch_bounds__(kBlock) k_scan(LOAD load, int64_t n, T *out, ScanState st) {
-    scan_tiles_loop<T, LOAD>(load, n, out, st);
-}
-
-// carve + reset the scan state out of the context workspace (after the partials area)
+// carve the scan slot out of the context workspace (after the partials area)
 static int scan_state(smcb_ctx *c, int64_t n, ScanState *st, int slot) {
     const size_t bytes = scan_state_bytes(n);
     const size_t base = (kWsPartials + 16) * sizeof(double);
     int rc = check_ws(c, base + 2 * bytes + 64);
     if (rc) return rc;
     const size_t half = ((c->ws_bytes - base) / 2) & ~(size_t)15;  // two slots: scans may chain
-    char *p = (char *)c->ws + base + (size_t)slot * half;
-    st->ticket = (unsigned int *)p;
-    st->agg = (unsigned long long *)(p + 16);
-    st->cpref = st->agg + scan_tiles(n);
-    SMCB_CUDA(cudaMemsetAsync(p, 0xFF, bytes, c->stream));
+    st->chunk_sum = (char *)c->ws + base + (size_t)slot * half;
     return SMCB_OK;
 }
 
@@ -464,22 +455,13 @@ __global__ void __launch_bounds__(kBlock) k_scan_chunks(LOAD load, int64_t n, in
     scan_chunks<T, LOAD>(load, n, tiles_per_chunk, chunk_sum, nchunks, out);
 }
 
-// reduce-then-scan (smcb_scan.cuh); `slot` 0 / 1: two scans may be in flight on the stream (multinomial, residual).
-// SMCB_SCAN_LOOKBACK=1 in the environment selects the single-pass look-back kernel instead.
+// reduce-then-scan (smcb_scan.cuh); `slot` 0 / 1: two scans may be in flight on the stream (multinomial, residual)
 template <typename T, typename LOAD>
 static int run_scan(smcb_ctx *c, const LOAD &load, int64_t n, T *out, int slot = 0) {
-    static const bool lookback = getenv("SMCB_SCAN_LOOKBACK") && atoi(getenv("SMCB_SCAN_LOOKBACK")) != 0;
     ScanState st;
     int rc = scan_state(c, n, &st, slot);
     if (rc) return rc;
     const int64_t tiles = scan_tiles(n);
-    if (lookback) {
-        int grid = (int)(tiles < kMaxGrid ? tiles : kMaxGrid);
-        k_scan<T, LOAD><<<grid, kBlock, 0, c->stream>>>(load, n, out, st);
-        c->launches++;
-        SMCB_CUDA(cudaGetLastError());
-        return SMCB_OK;
-    }
     // one chunk per CTA that can be resident (occupancy of the scan kernel x SMs): a grid of 1.1 - 1.4 waves, as the
     // fixed "6 per SM" gave, ends with a half-empty second round
     static int occ = 0;
@@ -492,7 +474,7 @@ static int run_scan(smcb_ctx *c, const LOAD &load, int64_t n, T *out, int slot =
     if (want > kScanMaxChunks) want = kScanMaxChunks;
     const int tpc = (int)((tiles + want - 1) / want);
     const int nchunks = (int)((tiles + tpc - 1) / tpc);
-    T *sums = reinterpret_cast<T *>(st.agg);                       // the slot's tile-state area doubles as the chunk sums
+    T *sums = reinterpret_cast<T *>(st.chunk_sum);
     k_scan_sums<T, LOAD><<<nchunks, kBlock, 0, c->stream>>>(load, n, tpc, sums);
     k_scan_chunks<T, LOAD><<<nchunks, kBlock, 0, c->stream>>>(load, n, tpc, sums, nchunks, out);
     c->launches += 2;

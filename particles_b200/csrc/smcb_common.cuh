@@ -14,7 +14,6 @@ constexpr int kBlock = 256;        // threads per CTA for the streaming kernels
 constexpr int kCtasPerSM = 8;      // 8 x 256 = 2048 resident threads / SM
 constexpr int kMaxGrid = kSMs * kCtasPerSM;
 constexpr double kHalfLog2Pi = 0.91893853320467274178;  // distributions.py:212
-constexpr unsigned long long kNotReady = 0xFFFFFFFFFFFFFFFFull;  // scan tile sentinel
 
 // ---------------------------------------------------------------------------
 // error plumbing
@@ -250,14 +249,14 @@ struct smcb_ctx {
     uint64_t seed;
     uint64_t api_counter;   // advances with every API-level random call
     int64_t launches;
-    double *ws;             // workspace: partials / tile status
+    double *ws;             // workspace: partials / scan slots
     size_t ws_bytes;
     unsigned int *counters; // "last block done" tickets (zeroed, self-resetting)
     double *math_tab;       // smcb_tables.h (64 KB): exp / log / sincos tables of the step kernels
 };
 
 namespace smcb {
-// workspace layout (doubles): [0, kWsPartials) block partials | 16 scalars | scan tile state
+// workspace layout (doubles): [0, kWsPartials) block partials | 16 scalars | two scan slots
 constexpr size_t kWsPartials = 65536;
 constexpr size_t kWsBytes = 8u << 20;  // 8 MiB: partials + up to ~1M scan tiles
 inline Philox key_of(uint64_t seed) {

@@ -11,18 +11,12 @@ int smcb_bind_1d_more(smcb_filter *f); // smcb_filter_1d.cu
 static int smcb_bind_1d(smcb_filter *f) {
     const smcb_filter_desc *d = &f->desc;
     switch (d->model) {
-#ifdef SMCB_BENCH_ONLY   // experiment builds: only the config-2 instantiation (fast compile)
-        case SMCB_MODEL_STOCHVOL:
-            return (d->fk == SMCB_FK_BOOTSTRAP && d->scheme == SMCB_RS_SYSTEMATIC)
-                       ? bind_one<StochVolM, SMCB_FK_BOOTSTRAP, SMCB_RS_SYSTEMATIC>(f) : SMCB_ENOSYS;
-#else
         case SMCB_MODEL_STOCHVOL: return bind_fk<StochVolM>(f);
         case SMCB_MODEL_LINGAUSS: return bind_fk<LinGaussM>(f);
         case SMCB_MODEL_GORDON:
         case SMCB_MODEL_THETALOGISTIC:
         case SMCB_MODEL_DISCRETECOX:
         case SMCB_MODEL_STOCHVOLLEV: return smcb_bind_1d_more(f);
-#endif
         default:
             set_error("fused filter: model id %d is not available in the fused 1-D family", d->model);
             return SMCB_ENOSYS;
@@ -30,9 +24,6 @@ static int smcb_bind_1d(smcb_filter *f) {
 }
 
 static int filter_setup(smcb_filter *f, smcb_ctx *c, const smcb_filter_desc *d);
-#ifdef SMCB_TRACE
-static unsigned long long *g_trace_buf = nullptr;
-#endif
 
 extern "C" int smcb_filter_create(smcb_ctx *c, const smcb_filter_desc *d, smcb_filter **out) {
     SMCB_REQUIRE(c && d && out, "smcb_filter_create: NULL argument");
@@ -85,14 +76,6 @@ static int filter_setup(smcb_filter *f, smcb_ctx *c, const smcb_filter_desc *d) 
     a.partials = reinterpret_cast<double *>(f->mem + kHdr);
     a.blk_agg = reinterpret_cast<double *>(f->mem + kHdr + part);
     a.math_tab = c->math_tab;
-    a.trace = nullptr;
-#ifdef SMCB_TRACE
-    if (!g_trace_buf) {
-        SMCB_CUDA(cudaMalloc(&g_trace_buf, sizeof(unsigned long long) * (8 * 256 + 32 * 256 + 64 * 256)));
-        SMCB_CUDA(cudaMemset(g_trace_buf, 0, sizeof(unsigned long long) * (8 * 256 + 32 * 256 + 64 * 256)));
-    }
-    a.trace = g_trace_buf;
-#endif
     a.X[0] = d->X[0]; a.X[1] = d->X[1]; a.lw[0] = d->lw[0]; a.lw[1] = d->lw[1];
     a.A = reinterpret_cast<long long *>(d->A);
     a.cdf = d->cdf;
@@ -113,7 +96,6 @@ static int filter_setup(smcb_filter *f, smcb_ctx *c, const smcb_filter_desc *d) 
         int dev = 0, sms = kSMs;
         SMCB_CUDA(cudaGetDevice(&dev));
         SMCB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        if (const char *e = getenv("SMCB_SMS")) { int v = atoi(e); if (v >= 1 && v < sms) sms = v; }   // experiments
         const int64_t npairs = (n + 1) / 2;
         int64_t g = sms < kMaxStepGrid ? sms : kMaxStepGrid;
         const int64_t gmax = (npairs + f->block_size - 1) / f->block_size;
@@ -140,7 +122,6 @@ static int filter_setup(smcb_filter *f, smcb_ctx *c, const smcb_filter_desc *d) 
             if (ns >= want) { n_small = ns < 0 ? 0 : (ns > n_iter / 8 ? n_iter / 8 : ns); break; }
         }
         if (n_small > n_iter) n_small = n_iter;
-        if (const char *e = getenv("SMCB_SLAB_IT")) { int v = atoi(e); if (v >= slab_it) slab_it = v; }   // experiments
         a.slab_it = (int)slab_it;
         a.slab_small = (int)n_small;
     }
@@ -350,13 +331,3 @@ extern "C" int smcb_p2p_free(void *dev_ptr) {
     if (dev_ptr) SMCB_CUDA(cudaFree(dev_ptr));
     return SMCB_OK;
 }
-
-#ifdef SMCB_TRACE
-// debug builds only (SMCB_NVCC_EXTRA=-DSMCB_TRACE, see build.py): timeline of the last step-kernel launch
-extern "C" int smcb_debug_trace(unsigned long long *host_out, int n_words) {
-    SMCB_CUDA(cudaDeviceSynchronize());
-    if (!g_trace_buf) return SMCB_EINVAL;
-    SMCB_CUDA(cudaMemcpy(host_out, g_trace_buf, sizeof(unsigned long long) * (size_t)n_words, cudaMemcpyDeviceToHost));
-    return SMCB_OK;
-}
-#endif

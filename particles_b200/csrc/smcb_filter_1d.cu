@@ -4,10 +4,6 @@
 #include "smcb_step.cuh"
 
 int smcb_bind_1d_more(smcb_filter *f) {
-#ifdef SMCB_BENCH_ONLY
-    set_error("experiment build: this model is not compiled in");
-    return SMCB_ENOSYS;
-#else
     switch (f->desc.model) {
         case SMCB_MODEL_GORDON: return bind_fk<GordonM>(f);
         case SMCB_MODEL_THETALOGISTIC: return bind_fk<ThetaLogisticM>(f);
@@ -17,5 +13,4 @@ int smcb_bind_1d_more(smcb_filter *f) {
             set_error("fused filter: model id %d is not available in the fused 1-D family", f->desc.model);
             return SMCB_ENOSYS;
     }
-#endif
 }

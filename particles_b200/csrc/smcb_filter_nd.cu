@@ -4,17 +4,6 @@
 
 int smcb_bind_nd(smcb_filter *f) {
     const smcb_filter_desc *d = &f->desc;
-#if defined(SMCB_BENCH_ND)      // experiment builds with the two config-3 instantiations (-DSMCB_BENCH_ND)
-    if (d->model == SMCB_MODEL_BEARINGS && d->fk == SMCB_FK_BOOTSTRAP && d->scheme == SMCB_RS_STRATIFIED)
-        return bind_one<BearingsM, SMCB_FK_BOOTSTRAP, SMCB_RS_STRATIFIED>(f);
-    if (d->model == SMCB_MODEL_MVLINGAUSS && d->dim == 4 && d->fk == SMCB_FK_GUIDED && d->scheme == SMCB_RS_STRATIFIED)
-        return bind_one<MvLinGaussM<4>, SMCB_FK_GUIDED, SMCB_RS_STRATIFIED>(f);
-    set_error("experiment build: only the config-3 instantiations are compiled in");
-    return SMCB_ENOSYS;
-#elif defined(SMCB_BENCH_ONLY)
-    set_error("experiment build: d-dimensional models are not compiled in");
-    return SMCB_ENOSYS;
-#else
     switch (d->model) {
         case SMCB_MODEL_BEARINGS:
             if (d->dim != 4) { set_error("fused BearingsOnly: state dimension must be 4"); return SMCB_EINVAL; }
@@ -29,5 +18,4 @@ int smcb_bind_nd(smcb_filter *f) {
             set_error("fused filter: model id %d has no d-dimensional kernel", d->model);
             return SMCB_ENOSYS;
     }
-#endif
 }

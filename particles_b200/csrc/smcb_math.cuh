@@ -24,41 +24,13 @@ namespace smcb {
 
 constexpr double kRintMagic = 6755399441055744.0;  // 1.5 * 2^52: x + magic rounds x to nearest int
 
-#ifndef SMCB_ESTRIN
-#define SMCB_ESTRIN 0
-#endif
-// polynomial evaluation: Horner (N-1 dependent FMAs) or Estrin (depth ~log2 N, a few more
-// multiplies) -- the latter shortens the dependent fp64 chains the step kernel waits on
+// polynomial evaluation (Horner: N-1 dependent FMAs)
 template <int N>
 __device__ __forceinline__ double horner(const double (&c)[N], double x) {
-#if SMCB_ESTRIN
-    constexpr int H = (N + 1) / 2;
-    double q[H];
-#pragma unroll
-    for (int i = 0; i < N / 2; i++) q[i] = fma(c[2 * i + 1], x, c[2 * i]);
-    if (N & 1) q[H - 1] = c[N - 1];
-    double xp = x * x;
-    int m = H;
-#pragma unroll
-    for (int level = 0; level < 5; level++) {
-        if (m > 1) {
-            const int h = (m + 1) / 2;
-#pragma unroll
-            for (int i = 0; i < H / 2 + 1; i++) {
-                if (i < m / 2) q[i] = fma(q[2 * i + 1], xp, q[2 * i]);
-            }
-            if (m & 1) q[h - 1] = q[m - 1];
-            xp = xp * xp;
-            m = h;
-        }
-    }
-    return q[0];
-#else
     double p = c[N - 1];
 #pragma unroll
     for (int i = N - 2; i >= 0; i--) p = fma(p, x, c[i]);
     return p;
-#endif
 }
 
 // exp(x): x <= ~709; returns 0 for x < -708 (incl. -inf; the lost range is < 3e-308),

@@ -1,17 +1,17 @@
-// smcb_scan.cuh -- single-pass inclusive prefix sum of non-negative fp64 values
+// smcb_scan.cuh -- inclusive prefix sum of non-negative fp64 (or int64) values
 // (the CDF walked by inverse_cdf, particles/resampling.py:484-509).
 //
-// Decoupled look-back (Merrill & Garland 2016) with two changes that make the
-// result a pure function of the input:
-//   * the exclusive prefix of tile t is DEFINED with a fixed (sequential) association over
-//     the tile aggregates:  P_0 = 0,  P_{t+1} = fl(P_t + a_t).  A tile takes the nearest
-//     already-published P_k as a shortcut and adds a_k .. a_{t-1} in order, so whichever k
-//     it finds, it computes the same bits: timing never changes the output.  Every tile
-//     publishes P_t and P_{t+1} as soon as it has them, so k is normally within a few tiles.
-//   * every level (thread, warp, block) clamps its values into the interval spanned by its
-//     own base and the base of its successor (tile level: [P_t, P_{t+1}]), which makes the
-//     output non-decreasing BY CONSTRUCTION.  np.searchsorted on it is then well defined and
-//     the search kernel can be held to it bit-exactly.
+// Reduce-then-scan.  The tiles of kScanTile values are grouped into <= kScanMaxChunks contiguous chunks, one CTA
+// each: pass 1 (scan_chunk_sums) sums every chunk, with no dependence between chunks; pass 2 (scan_chunks) lets
+// every CTA derive its chunk's base from the chunk sums and scan its chunk tile by tile with a local carry.  One
+// more read of the input than a single-pass scan (3 N instead of 2 N words of traffic), but no serial chain of
+// dependent global round trips over all tiles.  Two properties make the result a pure function of the input:
+//   * every association order is fixed: the chunk bases come from one CTA-wide scan of the chunk sums in a fixed
+//     order (identical bits in every CTA), and inside a chunk the tile bases are P_{t+1} = fl(P_t + a_t) in tile
+//     order.  Timing and scheduling never change the output.
+//   * every level (thread, warp, tile, chunk) clamps its values into the interval spanned by its own base and the
+//     base of its successor, which makes the output non-decreasing BY CONSTRUCTION.  np.searchsorted on it is then
+//     well defined and the search kernel can be held to it bit-exactly.
 #pragma once
 #include "smcb_common.cuh"
 
@@ -21,34 +21,18 @@ constexpr int kScanItems = 8;                       // fp64 values per thread
 constexpr int kScanTile = kBlock * kScanItems;      // 2048 values per tile
 
 
-struct ScanState {          // lives in the context workspace, reset to 0xFF.. per launch
-    unsigned int *ticket;   // dynamic tile id (starts at 0xFFFFFFFF -> first tile is 0)
-    unsigned long long *agg;   // [tiles]     tile aggregates a_t (bit pattern)
-    unsigned long long *cpref; // [tiles + 1] exclusive tile prefixes P_t
+struct ScanState {          // a scan slot of the context workspace
+    void *chunk_sum;        // [<= kScanMaxChunks] chunk sums of pass 1
 };
 
 inline int64_t scan_tiles(int64_t n) { return (n + kScanTile - 1) / kScanTile; }
+// bytes the context workspace reserves per scan slot (it grows with the tile count; run_search keeps its tile
+// bounds in slot 0)
 inline size_t scan_state_bytes(int64_t n) {
     int64_t t = scan_tiles(n);
     return 16 + 8 * (size_t)t + 8 * (size_t)(t + 2);
 }
 
-__device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned long long *p) {
-    return *reinterpret_cast<const volatile unsigned long long *>(p);
-}
-__device__ __forceinline__ unsigned long long canon_bits(double v) {
-    if (v != v) return 0x7FF8000000000000ull;  // canonical NaN can never equal the sentinel
-    return (unsigned long long)__double_as_longlong(v);
-}
-// int64 scans (offspring counts of residual resampling): values >= 0, never all-ones
-__device__ __forceinline__ unsigned long long canon_bits(long long v) { return (unsigned long long)v; }
-template <typename T> __device__ __forceinline__ T from_bits(unsigned long long b);
-template <> __device__ __forceinline__ double from_bits<double>(unsigned long long b) {
-    return __longlong_as_double((long long)b);
-}
-template <> __device__ __forceinline__ long long from_bits<long long>(unsigned long long b) {
-    return (long long)b;
-}
 template <typename T> __device__ __forceinline__ T tmin(T a, T b) { return b < a ? b : a; }
 template <typename T> __device__ __forceinline__ T tmax(T a, T b) { return a < b ? b : a; }
 __device__ __forceinline__ void store_items(double *out, int64_t i0, const double (&o)[8]) {
@@ -77,117 +61,10 @@ __device__ __forceinline__ T warp_scan_monotone(T v, int lane) {
     return v;
 }
 
-// LOAD: struct with  __device__ void operator()(int64_t i0, int64_t n, T (&v)[8]) const
-// filling v[j] with the value at index i0 + j (0 beyond n).  T = double or long long.
-template <typename T, typename LOAD>
-__device__ __forceinline__ void scan_tiles_loop(const LOAD &load, int64_t n, T *out,
-                                               ScanState st) {
-    __shared__ T s_warp[kBlock / 32];
-    __shared__ T s_pref[2];
-    __shared__ unsigned int s_tile;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const unsigned int ntiles = (unsigned int)((n + kScanTile - 1) / kScanTile);
-
-    for (;;) {
-        if (tid == 0) s_tile = atomicAdd(st.ticket, 1u) + 1u;
-        __syncthreads();
-        const unsigned int tile = s_tile;
-        if (tile >= ntiles) break;
-        const int64_t i0 = (int64_t)tile * kScanTile + (int64_t)tid * kScanItems;
-
-        T r[kScanItems];
-        load(i0, n, r);
-#pragma unroll
-        for (int j = 1; j < kScanItems; j++) r[j] = r[j - 1] + r[j];  // thread-local running sums
-
-        // block scan of the thread totals
-        T iw = warp_scan_monotone(r[kScanItems - 1], lane);
-        if (lane == 31) s_warp[warp] = iw;
-        __syncthreads();
-        T woff = 0;
-#pragma unroll
-        for (int w = 0; w < kBlock / 32; w++)
-            if (w < warp) woff = woff + s_warp[w];
-        T incl = woff + iw;                                  // I_k
-        T up = __shfl_up_sync(0xffffffffu, iw, 1);
-        T excl = (lane == 0) ? woff : (woff + up);           // E_k = I_{k-1}
-        if (tid == kBlock - 1)                                    // publish the tile aggregate
-            *reinterpret_cast<volatile unsigned long long *>(st.agg + tile) = canon_bits(incl);
-
-        // look-back: warp 0 obtains this tile's exclusive prefix P_t and P_{t+1} = fl(P_t + a_t)
-        if (warp == 0) {
-            T c = 0;
-            if (tile > 0) {
-                // (1) nearest published prefix P_k, k <= tile (P_0 = 0 by definition); lane l probes
-                //     index base - l, several windows back if need be
-                long long k = 0;
-                for (long long base = (long long)tile;; base -= 32) {
-                    const long long idx = base - lane;
-                    unsigned long long b = kNotReady;
-                    if (idx >= 1) b = ld_volatile_u64(st.cpref + idx);
-                    else if (idx == 0) b = canon_bits((T)0);
-                    const unsigned int ready = __ballot_sync(0xffffffffu, b != kNotReady);
-                    if (ready) {
-                        const int first = __ffs(ready) - 1;      // smallest lane = largest index
-                        k = base - first;
-                        c = from_bits<T>(__shfl_sync(0xffffffffu, b, first));
-                        break;
-                    }
-                }
-                // (2) c = (((P_k + a_k) + a_{k+1}) + ...) + a_{tile-1}: strictly sequential adds
-                for (long long j0 = k; j0 < (long long)tile; j0 += 32) {
-                    const long long j = j0 + lane;
-                    unsigned long long b = 0ull;
-                    if (j < (long long)tile) {
-                        do { b = ld_volatile_u64(st.agg + j); } while (b == kNotReady);
-                    }
-                    const T aj = from_bits<T>(b);
-                    const int cnt = (int)(((long long)tile - j0) < 32 ? ((long long)tile - j0) : 32);
-                    for (int l = 0; l < cnt; l++) c = c + __shfl_sync(0xffffffffu, aj, l);
-                }
-            }
-            T own = 0;                                // own aggregate: same association as `incl`
-#pragma unroll                                        // of thread kBlock-1, no global round trip
-            for (int w = 0; w < kBlock / 32; w++) own = own + s_warp[w];
-            own = from_bits<T>(canon_bits(own));
-            const T p_next = c + own;
-            if (lane == 0) {
-                s_pref[0] = c;
-                s_pref[1] = p_next;
-                if (tile > 0)
-                    *reinterpret_cast<volatile unsigned long long *>(st.cpref + tile) = canon_bits(c);
-                *reinterpret_cast<volatile unsigned long long *>(st.cpref + tile + 1) = canon_bits(p_next);
-            }
-        }
-        __syncthreads();
-        const T p_t = s_pref[0], p_next = s_pref[1];
-        const T base = p_t + excl;
-        const T cap = tmin(p_t + incl, p_next);
-        T o[kScanItems];
-#pragma unroll
-        for (int j = 0; j < kScanItems; j++) o[j] = tmin(base + r[j], cap);
-        if (i0 + kScanItems <= n) {
-            store_items(out, i0, o);
-        } else {
-#pragma unroll
-            for (int j = 0; j < kScanItems; j++)
-                if (i0 + j < n) out[i0 + j] = o[j];
-        }
-        __syncthreads();  // s_tile / s_pref / s_warp are reused by the next tile
-    }
-}
-
-// ---------------------------------------------------------------------------
-// Reduce-then-scan (the default of the stand-alone prefix sums).  The single-pass look-back above defines the tile
-// prefixes with ONE sequential chain over all tiles, P_{t+1} = fl(P_t + a_t): 4883 dependent global round trips at
-// N = 1e7, 167 us for 160 MB (0.15 of the HBM rate).  Here the tiles are grouped into <= 1024 contiguous chunks:
-// pass 1 sums each chunk (no dependence at all), pass 2 lets every CTA derive its chunk's base from the chunk sums
-// (fixed order: identical bits in every CTA) and scan its chunk tile by tile with a local carry.  Every level clamps
-// into [own base, successor's base] as before, so the output is non-decreasing by construction and a pure function
-// of the input.  One more read of the input (3 N instead of 2 N words of traffic), no serial chain.
-// ---------------------------------------------------------------------------
 constexpr int kScanMaxChunks = 4 * kBlock;          // the chunk-sum prefix is taken by one CTA-wide scan, 4 per thread
 
+// LOAD: struct with  __device__ void operator()(int64_t i0, int64_t n, T (&v)[8]) const
+// filling v[j] with the value at index i0 + j (0 beyond n).  T = double or long long.
 template <typename T, typename LOAD>
 __device__ __forceinline__ void scan_chunk_sums(const LOAD &load, int64_t n, int tiles_per_chunk, T *chunk_sum) {
     __shared__ T s_w[kBlock / 32];

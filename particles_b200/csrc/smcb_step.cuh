@@ -17,7 +17,6 @@
 //
 // The step index is a kernel argument (the host mirrors it); everything else a step needs from its
 // predecessor is in the partials (double-buffered by step parity) and in S_{t-2}.
-#include <limits.h>
 #include <string.h>
 
 #include <new>
@@ -39,44 +38,27 @@ constexpr int kMailScan = 17;       // slot[17] = t + 1 once the sender's CDF of
 constexpr int kMaxStepGrid = 256;   // CTAs of the step kernel: ONE per SM (132 on an H100), each owning a contiguous range
 constexpr int kMaxD = 4;
 constexpr int kTailBlock = 256;     // threads of the one-CTA helper kernels (>= kMaxStepGrid: one partial row per thread)
-// threads per CTA of the step kernel.  One CTA per SM: the warp scheduler favours the oldest CTA / warps
-// (with 3 equal CTAs per SM the first retires long before the last, the SM running few warps for the final
-// stretch), so all warps of an SM live in one CTA and pace each other (progress throttle in the streaming loop).
-#ifndef SMCB_KU
-#define SMCB_KU 2                // pairs of particles in flight per thread in the streaming branch (1-D states)
-#endif
-#ifndef SMCB_SCAN_GROUPS
-#define SMCB_SCAN_GROUPS 2       // warps per pipeline group of the resampling scan (0: the whole CTA scans one tile)
-#endif
 #ifndef SMCB_SPECULATE
 #define SMCB_SPECULATE 1         // sharded filters: start the streaming pass before the peers' statistics arrive
 #endif
-#ifndef SMCB_RS_PIPE
-#define SMCB_RS_PIPE 0             // resampling move pass of the 1-D models: hints two rounds ahead, CDF entries one
-#endif
-#ifndef SMCB_RS_KR
-#define SMCB_RS_KR 2             // resampling move pass: pairs in flight per thread
-#endif
-#ifndef SMCB_L2PREF
-#define SMCB_L2PREF 0            // streaming branch: iterations ahead whose input lines are prefetched into L2 (0: off)
-#endif
-#ifndef SMCB_SLAB_RECORDS
-#define SMCB_SLAB_RECORDS 128    // slab records (768 B each) in shared memory: 128 = the 96 KB of the CDF staging buffers
-#endif
-#ifndef SMCB_BS1D
-#define SMCB_BS1D 512            // threads per CTA of the step kernel for 1-D states (one CTA per SM): 16 warps at
-                                 // up to 128 registers beat 24 warps at 80 (which spill once the prefetch is on)
-#endif
 template <class M> struct StepCfg {
-    static constexpr int BS = (M::D == 1) ? SMCB_BS1D : 512;
-    static constexpr int kU = (M::D == 1) ? SMCB_KU : 1;   // d-dimensional states: one pair per thread (registers, and
-                                                            // a finer work unit for the N = 1e6 runs they are used at)
+    // threads per CTA of the step kernel.  One CTA per SM: the warp scheduler favours the oldest CTA / warps (with 3
+    // equal CTAs per SM the first retires long before the last, the SM running few warps for the final stretch), so
+    // all warps of an SM live in one CTA.  16 warps at up to 128 registers beat 24 warps at 80 (which spill once the
+    // prefetch is on).
+    static constexpr int BS = 512;
+    static constexpr int kU = (M::D == 1) ? 2 : 1;    // pairs in flight per thread in the streaming branch (d-dimensional
+                                                      // states: one -- registers, and a finer work unit for the N = 1e6
+                                                      // runs they are used at)
     static constexpr int kStage = 8 * BS;             // doubles of CDF staged per output tile (2 BS outputs)
     // dynamic shared memory: the math tables (smcb_tables.h, 64 KB), then two CDF slices (resampling branch) which
     // the streaming branch reuses for its slab records
-    static constexpr int kSlabDoubles = SMCB_SLAB_RECORDS * 96;   // per-lane slab records of the streaming branch
+    static constexpr int kSlabRecords = 128;          // slab records (768 B each): the 96 KB of the CDF staging buffers
+    static constexpr int kSlabDoubles = kSlabRecords * 96;   // per-lane slab records of the streaming branch
     static constexpr size_t dyn_smem = kMathTabBytes + (size_t)(2 * kStage > kSlabDoubles ? 2 * kStage : kSlabDoubles) * sizeof(double);
 };
+constexpr int kScanGroupWarps = 2;  // warps per pipeline group of the resampling scan (scan_scatter_groups)
+constexpr int kMovePairs = 2;       // resampling move pass: pairs in flight per thread
 
 // S_t: what is known once step t is finalised; st[t & 1]
 struct StepState {
@@ -106,7 +88,6 @@ struct FilterArgs {
     unsigned long long *bar; // grid-barrier arrivals, never reset
     double *blk_agg;         // multinomial: per-CTA sums of the exponential spacings (grid + 1)
     const double *math_tab;  // smcb_tables.h, built at context creation
-    unsigned long long *trace;   // SMCB_TRACE builds: per-CTA timeline of the last launch (else NULL, unused)
     int slab_it;             // iterations per slab of the streaming branch (host: chosen so the records fit)
     int slab_small;          // trailing iterations of a CTA's range handed out as single-iteration slabs
     int slab_lane;           // 1: a slab record holds the 32 lanes' own (m, s, q) (96 doubles); 0: their warp reduction
@@ -129,26 +110,6 @@ struct FilterArgs {
     const double *pX[8][2];
     const double *pcdf[8];
 };
-
-#ifdef SMCB_TRACE
-// per-CTA timeline of the LAST launch of the step kernel: {start, dependency resolved, prologue done, main loop
-// done, exit, smid} in ns (8 words per CTA), then per warp the time its main loop ended
-__device__ __forceinline__ unsigned long long gtimer() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    return t;
-}
-__device__ __forceinline__ unsigned int smid() {
-    unsigned int r;
-    asm volatile("mov.u32 %0, %smid;" : "=r"(r));
-    return r;
-}
-#define SMCB_TRACE_MARK(slot) do { if (threadIdx.x == 0) a.trace[8 * blockIdx.x + (slot)] = gtimer(); } while (0)
-#define SMCB_TRACE_WARP() do { if ((threadIdx.x & 31) == 0) a.trace[8 * 256 + 32 * blockIdx.x + (threadIdx.x >> 5)] = gtimer(); } while (0)
-#else
-#define SMCB_TRACE_MARK(slot) do { } while (0)
-#define SMCB_TRACE_WARP() do { } while (0)
-#endif
 
 __device__ __forceinline__ void wait_epoch(const volatile double *flag, double epoch, int *timeout) {
     const long long t0 = clock64();
@@ -302,10 +263,7 @@ __device__ __forceinline__ void acc_add_batch(Acc<D> &a, const double (&v)[NV], 
 
 struct StepSmem {
     double red[32 * 16];
-    int prog[32];
-    int next;                 // next slab / iteration of the streaming branch
-    int qn;                   // heavy entries queued by the scatter of a scan tile
-    long long q[64][3];
+    int next;                 // next slab of the streaming branch
     // pipelined scan (scan_scatter_groups): prefix ring, per-group warp totals / prefixes / heavy-entry queues
     double ringP[32];
     int ringF[32];
@@ -571,7 +529,6 @@ __device__ __forceinline__ bool prologue_begin(const FilterArgs &a, long long t,
     }
     double loc[16];
     shard_totals<APF>(a, s, pc.mom, sh, loc);
-    SMCB_TRACE_MARK(6);
     if (tid == 0) {
 #pragma unroll
         for (int i = 0; i < 16; i++) sh.carry[i] = loc[i];
@@ -685,7 +642,6 @@ __device__ __forceinline__ StepDecision prologue_end(const FilterArgs &a, long l
             }
         }
     }
-    SMCB_TRACE_MARK(7);
     if (d.rs && need_prefix) {
         // The CTAs own contiguous particle ranges, so their partial sums ARE the tile aggregates of the weight
         // scan: exclusive prefixes P_0 = 0 <= P_1 <= ... <= P_G (fixed order, monotone, the same bits in every
@@ -931,114 +887,17 @@ struct Scatter {
     }
 };
 
-constexpr int kHeavy = 48;          // offspring of one entry above which the whole CTA fills them cooperatively
-constexpr int kHeavyQ = 64;
-
-template <int BS, class LOAD>
-__device__ __forceinline__ void scan_scatter_range(const LOAD &load, int64_t e0, int64_t e1, double p_b, double p_next,
-                                                   double *out, double *s_warp, const Scatter &sc, bool last_cta,
-                                                   StepSmem &sh, int *s_hint, int hint_cap) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    constexpr int kTile = BS * kScanItems;
-    double carry = 0.0;
-    typename LOAD::Raw nxt;                                   // the next tile's loads are in flight while this one is scanned
-    load.fetch(e0 + (int64_t)tid * kScanItems, e1, nxt);
-    for (int64_t base0 = e0; base0 < e1; base0 += kTile) {
-        const int64_t i0 = base0 + (int64_t)tid * kScanItems;
-        const bool last_tile = base0 + kTile >= e1;
-        double r[kScanItems];
-        const typename LOAD::Raw cur = nxt;
-        if (!last_tile) load.fetch(i0 + kTile, e1, nxt);
-        load.weights(cur, i0, e1, r);
-#pragma unroll
-        for (int j = 1; j < kScanItems; j++) r[j] = r[j - 1] + r[j];
-        const double iw = warp_scan_monotone(r[kScanItems - 1], lane);
-        if (lane == 31) s_warp[warp] = iw;
-        if (tid == 0) sh.qn = 0;
-        __syncthreads();
-        double woff = 0.0, total = 0.0;
-#pragma unroll
-        for (int w = 0; w < BS / 32; w++) {
-            if (w < warp) woff = woff + s_warp[w];
-            total = total + s_warp[w];
-        }
-        const double incl = woff + iw;
-        const double up = __shfl_up_sync(0xffffffffu, iw, 1);
-        const double excl = (lane == 0) ? woff : (woff + up);
-        const double b_i = fmin(p_b + carry, p_next);         // base of this sub-tile
-        const double carry_next = carry + total;
-        const double b_next = fmin(p_b + carry_next, p_next); // base of the next one
-        const double tb = b_i + excl;
-        const double cap = fmin(b_i + incl, b_next);
-        double o[kScanItems];
-#pragma unroll
-        for (int j = 0; j < kScanItems; j++) o[j] = fmin(tb + r[j], cap);
-        if (i0 + kScanItems <= e1) {
-            store_items(out, i0, o);
-        } else {
-#pragma unroll
-            for (int j = 0; j < kScanItems; j++)
-                if (i0 + j < e1) out[i0 + j] = o[j];
-        }
-        // ---- scatter.  The tile's entries cover the outputs [K0, K1) = [F(b_i), F(b_next)) (the same fp64 expressions
-        // the neighbouring tiles / CTAs use, so coverage is gap-free).  Normally that range fits the shared-memory hint
-        // buffer: every thread writes the (tile-relative) entry index of each of its outputs there -- 4-byte stores with
-        // neighbouring lanes writing neighbouring words -- and the CTA then copies the buffer to A with fully coalesced
-        // 16-byte stores.  A range too long for the buffer (a few entries with very many offspring) is written directly.
-        const bool cta_tail = last_tile;                            // this tile ends the CTA's range
-        const long long K0 = (blockIdx.x == 0 && base0 == 0) ? 0 : sc.F(b_i);
-        const long long K1 = (cta_tail && last_cta) ? sc.n_out : sc.F(cta_tail ? p_next : b_next);
-        const bool staged = (K1 - K0) <= (long long)hint_cap;
-        if (i0 < e1) {
-            const bool tail_thread = (i0 + kScanItems >= e1);       // owns the last entry of the CTA's range
-            long long ks = (tid == 0) ? K0 : sc.F(tb);              // tb of thread 0 is b_i
-            const long long kend = (tid == BS - 1 || tail_thread) ? K1 : sc.F(b_i + incl);
-            ks = ks < K0 ? K0 : (ks > K1 ? K1 : ks);
-#pragma unroll
-            for (int j = 0; j < kScanItems; j++) {
-                if (i0 + j < e1) {
-                    const bool last_entry = (j == kScanItems - 1) || (i0 + j + 1 >= e1);
-                    long long ke = last_entry ? kend : sc.F(o[j]);
-                    ke = ke < ks ? ks : (ke > kend ? kend : ke);
-                    if (staged) {
-                        const int rel = tid * kScanItems + j;
-                        for (long long k = ks; k < ke; k++) s_hint[(int)(k - K0)] = rel;
-                    } else {
-                        if (ke - ks > kHeavy) {
-                            const int q = atomicAdd(&sh.qn, 1);
-                            if (q < kHeavyQ) { sh.q[q][0] = ks; sh.q[q][1] = ke; sh.q[q][2] = i0 + j; ks = ke; }
-                        }
-                        for (long long k = ks; k < ke; k++) sc.A[k] = i0 + j;
-                    }
-                    ks = ke;
-                }
-            }
-        }
-        carry = carry_next;
-        __syncthreads();
-        if (staged) {                                               // shared memory -> A, coalesced
-            const int cnt = (int)(K1 - K0);
-            for (int k = tid; k < cnt; k += BS) sc.A[K0 + k] = base0 + s_hint[k];
-        } else {
-            const int nq = sh.qn < kHeavyQ ? sh.qn : kHeavyQ;       // heavy entries: all threads fill their offspring
-            for (int q = 0; q < nq; q++) {
-                const long long ks = sh.q[q][0], ke = sh.q[q][1], jj = sh.q[q][2];
-                for (long long k = ks + tid; k < ke; k += BS) sc.A[k] = jj;
-            }
-        }
-        __syncthreads();
-    }
-}
+constexpr int kHeavy = 48;          // offspring of one entry above which the whole group fills them cooperatively
 
 // ---------------------------------------------------------------------------
-// The same scan + scatter as a PIPELINE of warp groups.  One CTA per SM means one block barrier domain per SM: with
-// the whole CTA on one tile every phase of the tile (loads, exponentials, warp scans, the prefix hand-over, stores)
-// is exposed -- measured 115 us for 16 B/particle where the three independent 256-thread CTAs of round 1 took 52.  So
-// the CTA's warps are split into NG groups of GW warps; group g takes the tiles g, g + NG, ... of the CTA's range, its
+// Scan + scatter of the CTA's range as a PIPELINE of warp groups.  One CTA per SM means one block barrier domain per
+// SM: with the whole CTA on one tile every phase of the tile (loads, exponentials, warp scans, the prefix hand-over,
+// stores) is exposed -- measured 115 us for 16 B/particle where the three independent 256-thread CTAs of round 1 took
+// 52.  So the CTA's warps are split into NG groups of GW warps; group g takes the tiles g, g + NG, ... of the CTA's range, its
 // own named barrier (bar.sync g + 1) and its own slice of the hint buffer; the only thing a tile needs from its
 // predecessor is the running prefix P_t, handed over through a small shared-memory ring (value + epoch flag) right
 // after the group's warp scan -- a decoupled look-back of depth one with a FIXED association order
-// (P_{t+1} = min(P_t + total_t, p_next)), so the CDF is deterministic and monotone by construction as before.
+// (P_{t+1} = min(P_t + total_t, p_next)), so the CDF is deterministic and monotone by construction.
 // ---------------------------------------------------------------------------
 constexpr int kScanRing = 32;
 constexpr int kGroupQ = 8;
@@ -1116,7 +975,13 @@ __device__ __forceinline__ void scan_scatter_groups(const LOAD &load, int64_t e0
             for (int j = 0; j < kScanItems; j++)
                 if (i0 + j < e1) out[i0 + j] = o[j];
         }
-        // scatter (see scan_scatter_range): [K0, K1) = [F(P_t), F(P_{t+1})), staged in the group's hint buffer
+        // ---- scatter.  The tile's entries cover the outputs [K0, K1) = [F(P_t), F(P_{t+1})) (the same fp64
+        // expressions the neighbouring tiles / CTAs use, so coverage is gap-free).  Normally that range fits the
+        // group's slice of the shared-memory hint buffer: every thread writes the (tile-relative) entry index of each
+        // of its outputs there -- 4-byte stores with neighbouring lanes writing neighbouring words -- and the group
+        // then copies the buffer to A with fully coalesced stores.  A range too long for the buffer (a few entries
+        // with very many offspring) is written directly; entries with more than kHeavy offspring are queued, and the
+        // whole group fills them cooperatively.
         const long long K0 = (blockIdx.x == 0 && t == 0) ? 0 : sc.F(b_i);
         const long long K1 = (last_tile && last_cta) ? sc.n_out : sc.F(last_tile ? p_next : b_next);
         const bool staged = (K1 - K0) <= (long long)hint_cap;
@@ -1224,17 +1089,6 @@ __device__ __forceinline__ int shard_of(const double *goff, const double *gpi, i
 // the step kernel: resample_move + reweight_particles (+ compute_summaries of the previous step)
 // (core.py:323-367)
 // ---------------------------------------------------------------------------
-#ifndef SMCB_THROTTLE
-#define SMCB_THROTTLE 1          // SMCB_SCHED 0: iterations a warp may run ahead of the slowest warp of its CTA (0: off)
-#endif
-#ifndef SMCB_PREFETCH
-#define SMCB_PREFETCH 1          // streaming branch, 1-D states: request the next iteration's inputs one iteration ahead
-                                 // (77.5 vs 80.8 us at 512 threads; at 768 threads / 80 registers it spills: 120 us)
-#endif
-#ifndef SMCB_SCHED
-#define SMCB_SCHED 2             // 0 static + throttle, 1 dynamic (experiment, order-dependent sums), 2 dynamic slabs
-#endif
-
 template <class M, int FK, int SCHEME>
 __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs a, long long t) {
     constexpr bool APF = FkTraits<FK>::apf;
@@ -1248,16 +1102,12 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
     __shared__ __align__(8) uint64_t s_tabbar;
     __shared__ long long s_hi;
     __shared__ double s_warp[BS / 32];
-#ifdef SMCB_TRACE
-    if (threadIdx.x == 0) { a.trace[8 * blockIdx.x] = gtimer(); a.trace[8 * blockIdx.x + 5] = smid(); }
-#endif
     // the tables are constants: their copy may start before the previous kernel has retired
     if (threadIdx.x == 0) { mtab_issue(a.math_tab, &s_tabbar); sh.next = 0; }
     // everything below reads what the previous kernel of the stream wrote (programmatic dependent launch:
     // this kernel may have been scheduled before its predecessor retired)
     cudaGridDependencySynchronize();
     cudaTriggerProgrammaticLaunchCompletion();
-    SMCB_TRACE_MARK(1);
     // Sharded filters with the mailbox exchange SPECULATE: a step whose shard-local ESS test says "no resampling"
     // starts its streaming pass at once and collects the peers' statistics afterwards -- the exchange latency (peer's
     // step end + NVLink store + fence + poll) leaves the critical path.  The pass writes only the other half of the
@@ -1274,7 +1124,6 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
     // (no block barrier on the speculative path: CTA 0's sending lanes sit in their system-scope fence for a few
     // microseconds, and the other warps of that CTA start on the slabs meanwhile -- the dynamic slab schedule absorbs it)
     mbar_wait(&s_tabbar, 0);                           // (the prologue's barriers made the init visible)
-    SMCB_TRACE_MARK(2);
     const int cur = (int)((t - 1) & 1);                // step s writes buffers [s & 1]
     const bool rs = dec.rs != 0;                       // (a speculative step enters the resampling branch from below)
     double reset_c = dec.reset_c;
@@ -1295,7 +1144,7 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
     Acc<D> acc;
     acc_init(acc);
     Lse3 aux = lse3_empty();
-    int n_slab = 0;                                    // slab records of the streaming branch (SMCB_SCHED 2)
+    int n_slab = 0;                                    // slab records of the streaming branch
 
     // propagate + reweight one pair of particles; writes x', lw'; returns x', lw' (and the auxiliary
     // log-weights of the next step for an APF), -inf in masked slots
@@ -1374,16 +1223,6 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
         };
         auto compute_full = [&](int i, const In &in, Acc<D> &ac, Lse3 &ax) {
             double l[2 * kU], av[APF ? 2 * kU : 1], x[2 * kU][D];
-#if SMCB_L2PREF
-            {   // pull the inputs some iterations ahead of the CTA's front into L2 (one line per lane, 1-D states)
-                const int ip = i + SMCB_L2PREF;
-                constexpr int kLines = kIt / 8;               // 128-byte lines per array and iteration
-                if (D == 1 && ip < n_full && lane < 2 * kLines) {
-                    const double *src = (lane < kLines ? lwi_c : Xi_c) + 2 * ((size_t)ip * kIt) + (size_t)(lane % kLines) * 16;
-                    asm volatile("prefetch.global.L2 [%0];" ::"l"(src));
-                }
-            }
-#endif
             bool odd = false;                                 // some value is +-inf / NaN (integer test)
 #pragma unroll
             for (int u = 0; u < kU; u++) {
@@ -1474,37 +1313,6 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
             acc_add_batch<2 * kU, D>(ac, l, x, mom);
             if (APF) lse3_add_batch<(APF ? 2 * kU : 1)>(ax, av);
         };
-#if SMCB_SCHED == 0
-        constexpr int NW = BS / 32;
-        const int warp = threadIdx.x >> 5;
-        // static round-robin of the iterations over the warps; the warps pace each other (none starts its
-        // (k + SMCB_THROTTLE + 1)-th iteration before all have finished their k-th)
-        if (threadIdx.x < 32) sh.prog[threadIdx.x] = (threadIdx.x < NW) ? 0 : INT_MAX;
-        __syncthreads();
-        int it = 0;
-        for (int i = warp; i < n_iter; i += NW) {
-            iteration(i, acc, aux);
-            it++;
-#if SMCB_THROTTLE
-            if (lane == 0) *reinterpret_cast<volatile int *>(&sh.prog[warp]) = it;
-            for (int spin = 0; spin < (1 << 16); spin++) {          // bounded: pacing is an optimisation only
-                const int mn = __reduce_min_sync(0xffffffffu, *reinterpret_cast<volatile int *>(&sh.prog[lane]));
-                if (mn >= it - SMCB_THROTTLE) break;
-                __nanosleep(100);
-            }
-#endif
-        }
-        if (lane == 0) *reinterpret_cast<volatile int *>(&sh.prog[warp]) = INT_MAX;    // done: nobody waits for this warp
-#elif SMCB_SCHED == 1
-        // EXPERIMENT: dynamic iterations, thread accumulators (summation order depends on the schedule)
-        for (;;) {
-            int i = 0;
-            if (lane == 0) i = atomicAdd(&sh.next, 1);
-            i = __shfl_sync(0xffffffffu, i, 0);
-            if (i >= n_iter) break;
-            iteration(i, acc, aux);
-        }
-#else
         // dynamic slabs: a warp takes the next slab of `slab_it` consecutive iterations from a shared counter, so
         // the warps of the SM drift apart (one warp's loads overlap the others' arithmetic) and all retire within
         // one slab of each other whatever the scheduler's priorities.  Determinism: a slab's statistics are parked in
@@ -1527,8 +1335,9 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
         };
         auto first_it = [&](int sl) { return sl < n_big ? sl * slab_it : it_small0 + (sl - n_big); };
         // software pipeline (1-D states): the inputs of the next iteration -- of this slab, or of the slab the warp
-        // takes next -- are requested before the current iteration's arithmetic starts
-        constexpr bool PREF = (D == 1) && (SMCB_PREFETCH != 0);
+        // takes next -- are requested before the current iteration's arithmetic starts (77.5 vs 80.8 us at 512
+        // threads; at 768 threads / 80 registers it spills: 120 us)
+        constexpr bool PREF = (D == 1);
         int sl = grab();
         In pre;
         bool have = false;
@@ -1559,8 +1368,6 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
             else warp_reduce_to_slab<D, APF>(sa, sx, mom, rec, lane);
             sl = nsl;
         }
-#endif
-        SMCB_TRACE_WARP();
         if (!speculate) goto step_done;
         // now the peers' statistics: bookkeeping, and was the guess right?
         __syncthreads();
@@ -1598,15 +1405,10 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
             const int64_t e1 = 2 * pend < n ? 2 * pend : n;
             if (count_path) {
                 Scatter sc{a.A, (double)n, (SCHEME == SMCB_RS_SYSTEMATIC) ? u_sys : 0.0, (long long)n};
-#if SMCB_SCAN_GROUPS
                 if (threadIdx.x == 0) sh.timeout_ptr = a.sync_timeout;
-                scan_scatter_groups<BS, SMCB_SCAN_GROUPS>(load, 2 * pstart, e1, dec.p_b, dec.p_next, a.cdf, sc,
-                                                          blockIdx.x == gridDim.x - 1, sh, reinterpret_cast<int *>(s_stage),
-                                                          4 * kStage);
-#else
-                scan_scatter_range<BS>(load, 2 * pstart, e1, dec.p_b, dec.p_next, a.cdf, s_warp, sc,
-                                       blockIdx.x == gridDim.x - 1, sh, reinterpret_cast<int *>(s_stage), 4 * kStage);
-#endif
+                scan_scatter_groups<BS, kScanGroupWarps>(load, 2 * pstart, e1, dec.p_b, dec.p_next, a.cdf, sc,
+                                                         blockIdx.x == gridDim.x - 1, sh, reinterpret_cast<int *>(s_stage),
+                                                         4 * kStage);
             } else {
                 scan_range<BS>(load, 2 * pstart, e1, dec.p_b, dec.p_next, a.cdf, s_warp);
             }
@@ -1617,10 +1419,8 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
             grid_barrier(a, bar_target);
             spacings_pass2<BS>(a, sh, s_warp);
         }
-        SMCB_TRACE_MARK(6);                                // (resampling step: scan + scatter done)
         bar_target += gridDim.x;
         grid_barrier(a, bar_target);
-        SMCB_TRACE_MARK(7);                                // (grid barrier passed)
         // shared tail of both searches: gather the ancestors' states, restart weights, propagate
         auto finish_pair = [&](int64_t p, const double *X0, const double *X1, int64_t a0, int64_t a1, long long g0,
                                long long g1, bool write_A = true) {
@@ -1701,18 +1501,9 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
                 }
                 return lo_;
             };
-            constexpr int kR = SMCB_RS_KR;                          // pairs in flight per thread
-#ifdef SMCB_TRACE
-            unsigned dbg_n = 0; long long dbg_d = 0;
-#endif
-#ifdef SMCB_TRACE
-            unsigned long long dbg_t[3] = {0, 0, 0};
-#endif
+            constexpr int kR = kMovePairs;                          // pairs in flight per thread
             // one round = kR pairs per thread, in three parts: the hints (A, written by the scan), the CDF entries that
-            // verify them, and verify + repair + gather + propagate.  The first two are plain loads with no arithmetic
-            // behind them, so for the 1-D models they are issued one / two rounds AHEAD (software pipeline): the move
-            // pass is a chain hint -> CDF -> gather -> fp64 work, and with 16 warps per SM the chain's latencies were
-            // not covered by the other warps' arithmetic (move pass 132 us against 78 us for the same arithmetic alone).
+            // verify them, and verify + repair + gather + propagate
             struct Hints { long long h[kR][2]; };
             struct Cdf { double c0[kR][2], cm[kR][2], c1[kR][(SCHEME == SMCB_RS_STRATIFIED) ? 2 : 1]; };
             auto ld_hints = [&](int64_t p0, Hints &H) {
@@ -1748,9 +1539,6 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
                 }
             };
             auto process = [&](int64_t p0, const Hints &H, const Cdf &Cc) {
-#ifdef SMCB_TRACE
-                const unsigned long long dbg_t1 = gtimer() + (unsigned long long)(Cc.c0[0][0] > 3.0);    // (after the loads)
-#endif
                 long long h[kR][2];
                 double su[kR][2];
                 bool valid[kR], two[kR], moved[kR];
@@ -1809,73 +1597,26 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
                             }
                         }
                         if (on && !ok) {
-#ifdef SMCB_TRACE
-                            const long long h_was = h[r][q];
-#endif
                             h[r][q] = settle(h[r][q], su[r][q]);
                             moved[r] = true;
-#ifdef SMCB_TRACE
-                            dbg_n++;
-                            const long long dd = h[r][q] > h_was ? h[r][q] - h_was : h_was - h[r][q];
-                            dbg_d = dd > dbg_d ? (dd > 0x7fffffffll ? 0x7fffffffll : dd) : dbg_d;
-#endif
                         }
                     }
                     if (!two[r]) h[r][1] = h[r][0];
                 }
-#ifdef SMCB_TRACE
-                const unsigned long long dbg_t2 = gtimer() + (unsigned long long)(h[0][0] < -5);
-#endif
 #pragma unroll
                 for (int r = 0; r < kR; r++) {
                     const int64_t p = p0 + (int64_t)r * BS;
                     if (valid[r]) finish_pair(p, Xi, Xi, h[r][0], h[r][1], h[r][0], h[r][1], moved[r]);
                 }
-#ifdef SMCB_TRACE
-                const unsigned long long dbg_t3 = gtimer() + (unsigned long long)(acc.w.s < -1.0);
-                dbg_t[1] = max(dbg_t[1], dbg_t2 - dbg_t1); dbg_t[2] = max(dbg_t[2], dbg_t3 - dbg_t2);
-#endif
             };
             constexpr int64_t kStep = (int64_t)kR * BS;
-            if (SMCB_RS_PIPE && D == 1) {
-                Hints h_cur, h_nxt;
-                Cdf c_cur;
-                int64_t p0 = pstart + threadIdx.x;
-                ld_hints(p0, h_cur);                                 // (all loaders mask pairs beyond pend themselves)
-                ld_hints(p0 + kStep, h_nxt);
-                ld_cdf(p0, h_cur, c_cur);
-                for (; p0 < pend; p0 += kStep) {
-                    Hints h_n2;
-                    Cdf c_nxt;
-                    ld_cdf(p0 + kStep, h_nxt, c_nxt);                // its hints were requested a round ago
-                    ld_hints(p0 + 2 * kStep, h_n2);
-                    process(p0, h_cur, c_cur);
-                    h_cur = h_nxt; c_cur = c_nxt; h_nxt = h_n2;
-                }
-            } else {
-                for (int64_t p0 = pstart + threadIdx.x; p0 < pend; p0 += kStep) {
-                    Hints H;
-                    Cdf Cc;
-                    ld_hints(p0, H);
-                    ld_cdf(p0, H, Cc);
-                    process(p0, H, Cc);
-                }
+            for (int64_t p0 = pstart + threadIdx.x; p0 < pend; p0 += kStep) {
+                Hints H;
+                Cdf Cc;
+                ld_hints(p0, H);
+                ld_cdf(p0, H, Cc);
+                process(p0, H, Cc);
             }
-#ifdef SMCB_TRACE
-            {   // per warp: end of its move loop | (settle calls << 32 | largest hint error) of the resampling step
-                const unsigned cnt = __reduce_add_sync(0xffffffffu, dbg_n);
-                const unsigned far = __reduce_max_sync(0xffffffffu, (unsigned)dbg_d);
-                if ((threadIdx.x & 31) == 0) {
-                    a.trace[8 * 256 + 32 * blockIdx.x + (threadIdx.x >> 5)] = gtimer();
-                    a.trace[8 * 256 + 32 * blockIdx.x + 16 + (threadIdx.x >> 5)] = ((unsigned long long)cnt << 32) | far;
-                }
-                // longest single round of this warp, by part: hint + CDF loads | settle | gather + propagate + reweight
-                for (int i = 0; i < 3; i++) {
-                    const unsigned v = __reduce_max_sync(0xffffffffu, (unsigned)dbg_t[i]);
-                    if ((threadIdx.x & 31) == 0) a.trace[40 * 256 + 64 * blockIdx.x + 4 * (threadIdx.x >> 5) + i] = v;
-                }
-            }
-#endif
         } else if (!a.rs_global) {
             const double M_ = (double)n;
             const double zlast = (SCHEME == SMCB_RS_MULTINOMIAL) ? __ldcg(a.su + n) : 1.0;
@@ -2092,9 +1833,7 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
         }
     }
 step_done:
-    SMCB_TRACE_MARK(3);
     write_partial<D, APF, BS>(a, t, acc, aux, mom, sh, s_stage, n_slab);
-    SMCB_TRACE_MARK(4);
 }
 
 // the prologue alone (one CTA): finalises the last enqueued step so that the host can read its summaries
