@@ -283,6 +283,46 @@ int smcb_filter_step_timed(smcb_filter *f, int64_t nsteps, double *out8);
  * [5]=log_mean_w, [6]=max lw, [7]=sum w */
 int smcb_filter_state(smcb_filter *f, double *out8);
 
+/* ---------------------------------------------------------------------------
+ * off-line smoothing: FFBS backward sampling over a stored history (particles/smoothing.py:278-423)
+ * ------------------------------------------------------------------------- */
+#define SMCB_SMOOTH_ON2 0    /* backward_sampling_ON2,    smoothing.py:291-311 */
+#define SMCB_SMOOTH_MCMC 1   /* backward_sampling_mcmc,   smoothing.py:313-350 */
+#define SMCB_SMOOTH_REJECT 2 /* backward_sampling_reject, smoothing.py:352-423 (hybrid, Dau & Chopin 2022) */
+#define SMCB_SMOOTH_GATHER 3 /* paths[t] = X[t][idx[t]] only (idx given; model ignored) */
+
+typedef struct {
+    int32_t method, model, dim, n_params;
+    int64_t T, N, M;
+    int64_t nsteps;            /* MCMC: Metropolis steps per time                                  */
+    int64_t max_trials;        /* reject: proposals per trajectory before the exact O(N) draw      */
+    double params[SMCB_MAX_PARAMS];  /* model constants, same layout as smcb_filter_desc.params    */
+    const double *step_consts; /* NULL, or (T) per-step model constants (Gordon_etal)              */
+    /* the history: device arrays of T device pointers; X[t] holds particle n, component c at
+       X[t][n * x_stride_n + c * x_stride_c] (element strides, the same for every t) */
+    const double *const *X;
+    const double *const *lw;   /* (N) log-weights per t                                             */
+    const int64_t *const *A;   /* (N) ancestors per t (entry 0 unused)                              */
+    int64_t x_stride_n, x_stride_c;
+    const double *log_bound;   /* reject: (T-1), entry t = log C_{t+1} >= log p(x_{t+1} | x_t)       */
+    const double *cdf;         /* MCMC / reject: (T-1, cdf_ld) rows, the inclusive prefix sums of W_t */
+    int64_t cdf_ld;            /* row stride of cdf (>= N; even, so that every row is 16-byte aligned) */
+    const int64_t *idx_T;      /* (M) the final-time indices (drawn by the caller)                  */
+    /* injected randomness (parity tests) or NULL -> Philox keyed by (seed, call, m, t, trial):
+       ON2 u (M, T-1) [m, t]; MCMC prop / lu (T-1, nsteps, M); reject prop / lu (T-1, M, max_trials)
+       and u_exact (T-1, M) for the exact fallback draw */
+    const double *u;
+    const int64_t *prop;
+    const double *lu;
+    const double *u_exact;
+    int64_t *idx;              /* out (T, M): idx[T-1] = idx_T; GATHER: input                       */
+    double *paths;             /* out (T, M, dim) = X[t][idx[t]]                                    */
+    int64_t *counts;           /* reject: out (T-1, 2) {accepted, proposals} (zeroed here)          */
+} smcb_smooth_desc;
+
+/* ONE kernel launch for the whole backward pass (plus a memset of counts for reject); no host sync */
+int smcb_backward_sample(smcb_ctx *ctx, const smcb_smooth_desc *desc);
+
 #ifdef __cplusplus
 }
 #endif

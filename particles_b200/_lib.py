@@ -38,6 +38,21 @@ class FilterDesc(C.Structure):
     ]
 
 
+SMOOTH_ON2, SMOOTH_MCMC, SMOOTH_REJECT, SMOOTH_GATHER = 0, 1, 2, 3
+
+
+class SmoothDesc(C.Structure):
+    _fields_ = [
+        ("method", C.c_int32), ("model", C.c_int32), ("dim", C.c_int32), ("n_params", C.c_int32),
+        ("T", C.c_int64), ("N", C.c_int64), ("M", C.c_int64), ("nsteps", C.c_int64), ("max_trials", C.c_int64),
+        ("params", C.c_double * SMCB_MAX_PARAMS), ("step_consts", c_dp),
+        ("X", c_dp), ("lw", c_dp), ("A", c_dp), ("x_stride_n", C.c_int64), ("x_stride_c", C.c_int64),
+        ("log_bound", c_dp), ("cdf", c_dp), ("cdf_ld", C.c_int64), ("idx_T", c_dp),
+        ("u", c_dp), ("prop", c_dp), ("lu", c_dp), ("u_exact", c_dp),
+        ("idx", c_dp), ("paths", c_dp), ("counts", c_dp),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/smcb.h declares
 PROTOTYPES = {
     "smcb_last_error": (C.c_char_p, []),
@@ -93,6 +108,7 @@ PROTOTYPES = {
     "smcb_p2p_free": (C.c_int, [C.c_void_p]),
     "smcb_filter_step_timed": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_double)]),
     "smcb_filter_state": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),
+    "smcb_backward_sample": (C.c_int, [C.c_void_p, C.POINTER(SmoothDesc)]),
 }
 
 _lib = None

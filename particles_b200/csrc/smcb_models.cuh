@@ -36,6 +36,17 @@ __device__ __forceinline__ double normal_logpdf_ls(double x, double loc, double 
     return -z * z / 2.0 - kHalfLog2Pi - logscale;
 }
 
+// log(sqrt(2 pi)) as scipy.stats.norm.logpdf holds it (np.log of the rounded sqrt): one ulp below the correctly
+// rounded kHalfLog2Pi.  The transition density of the backward samplers uses it so that PX.logpdf is bit-identical
+// to the reference's.
+constexpr double kHalfLog2PiScipy = 0x1.d67f1c864beb4p-1;
+
+// x / c with r = RN(1 / c): the correctly rounded quotient (see MvLinGaussM::div_const)
+__host__ __device__ __forceinline__ double div_rn(double x, double c, double r) {
+    const double q = x * r;
+    return fma(fma(-q, c, x), r, q);
+}
+
 // ---------------------------------------------------------------------------
 // StochVol -- particles/state_space_models.py:446-498
 // params: 0 mu, 1 rho, 2 sigma, 3 sig0, 4 (1-rho)*mu, 5 log(sigma), 6 log(sig0)
@@ -286,14 +297,26 @@ __device__ __forceinline__ void fk_move(const M &m, const StepK &k, double xp, d
 // BearingsOnly -- particles/state_space_models.py:580-608 (Bootstrap only: the reference defines
 // no proposal).  State (x0, x1, x2, x3); PX = IndepProd(N(x0, sX), N(x1, sX), Dirac(x0 + x2),
 // Dirac(x1 + x3)); PY = Normal(arctan(x3 / x2) [+ pi if x2 < 0], sY).
-// params: 0 sigmaX, 1 sigmaY, 2 log sigmaY, 3..6 x0[4]
+// params: 0 sigmaX, 1 sigmaY, 2 log sigmaY, 3..6 x0[4], 7 log sigmaX (transition density only)
 struct BearingsM {
     static constexpr int D = 4, NZ = 2;
     static constexpr bool has_proposal = false;
-    double sX, sY, lsY, x0[4];
+    double sX, sY, lsY, x0[4], lsX, isX;
     __host__ void load(const double *p) {
         sX = p[0]; sY = p[1]; lsY = p[2];
         for (int i = 0; i < 4; i++) x0[i] = p[3 + i];
+        lsX = p[7]; isX = 1.0 / sX;
+    }
+    // PX(t, xp).logpdf(x): IndepProd of N(xp0, sX), N(xp1, sX), Dirac(xp0 + xp2), Dirac(xp1 + xp3), summed in
+    // component order (distributions.py IndepProd.logpdf); a Dirac gives 0 where x == loc, -inf elsewhere
+    __device__ __forceinline__ void trans_loc(const StepK &, const double *xp, double *lc) const {
+        lc[0] = xp[0]; lc[1] = xp[1]; lc[2] = xp[0] + xp[2]; lc[3] = xp[1] + xp[3];
+    }
+    __device__ __forceinline__ double trans_lpdf(const double *lc, const double *x) const {
+        const double z0 = div_rn(x[0] - lc[0], sX, isX), z1 = div_rn(x[1] - lc[1], sX, isX);
+        const double a = -z0 * z0 / 2.0 - kHalfLog2PiScipy - lsX, b = -z1 * z1 / 2.0 - kHalfLog2PiScipy - lsX;
+        const double c = (x[2] == lc[2]) ? 0.0 : -CUDART_INF, d = (x[3] == lc[3]) ? 0.0 : -CUDART_INF;
+        return ((a + b) + c) + d;
     }
     __device__ __forceinline__ double obs(const StepK &k, const double *x) const {   // :603-608
         double angle = atan(x[3] / x[2]);
@@ -459,7 +482,61 @@ struct MvLinGaussM {
         matvec_G(pm, gy);
         return logpdf_y(k.yn, gy, LE, iLE, hldE);
     }
+    // PX(t, xp).logpdf(x) = MvNormal(F xp, covX).logpdf(x), kalman.py:339-340
+    __device__ __forceinline__ void trans_loc(const StepK &, const double *xp, double *lc) const { matvec_F(xp, lc); }
+    __device__ __forceinline__ double trans_lpdf(const double *lc, const double *x) const {
+        return logpdf_x(x, lc, LX, iLX, hldX);
+    }
 };
+
+// ---------------------------------------------------------------------------
+// transition density PX(t, xp).logpdf(x) (Bootstrap.logpt, state_space_models.py:341-342) for backward sampling
+// (csrc/smcb_smooth.cu).  `k` carries the time of x: logpt(t + 1, X_t, x_{t+1}) is evaluated with k.t = t + 1 and
+// Gordon's step constant of t + 1.  Split in two so that the O(N^2) sampler computes the per-ancestor part once
+// and shares it over every trajectory: loc(k, xp) -> D values, then lpdf(loc, x) per pair.
+// ---------------------------------------------------------------------------
+// models whose PX calls mexp (the table family): a kernel evaluating their density stages the tables first
+template <class M> struct TransUsesTable { static constexpr bool value = false; };
+template <> struct TransUsesTable<ThetaLogisticM> { static constexpr bool value = true; };
+
+template <class M>
+struct TransDensity {
+    double s, is, ls;   // 1-D models: the (constant) scale of PX, its reciprocal and its log
+    __device__ __forceinline__ void init(const M &m) {
+        if constexpr (M::D == 1) {
+            StepK k{};
+            double l;
+            m.trans(k, 0.0, l, s, ls);
+            is = 1.0 / s;
+        }
+    }
+    __device__ __forceinline__ void loc(const M &m, const StepK &k, const double *xp, double *lc) const {
+        if constexpr (M::D == 1) {
+            double sc, l;
+            m.trans(k, xp[0], lc[0], sc, l);
+        } else {
+            m.trans_loc(k, xp, lc);
+        }
+    }
+    // Normal.logpdf in the reference's order: z = (x - loc) / scale, -z^2/2 - log(2 pi)/2 - log(scale)
+    __device__ __forceinline__ double lpdf(const M &m, const double *lc, const double *x) const {
+        if constexpr (M::D == 1) {
+            const double z = div_rn(x[0] - lc[0], s, is);
+            return -z * z / 2.0 - kHalfLog2PiScipy - ls;
+        } else {
+            return m.trans_lpdf(lc, x);
+        }
+    }
+};
+
+template <class M>
+__device__ __forceinline__ double trans_logpdf(const M &m, const StepK &k, const double *xp, const double *x) {
+    TransDensity<M> td;
+    td.init(m);
+    double lc[M::D];
+    td.loc(m, k, xp, lc);
+    return td.lpdf(m, lc, x);
+}
 
 // uniform entry points for the step kernels: scalar Normal-kernel models or vector models
 template <class M, int FK>

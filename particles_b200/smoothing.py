@@ -1,16 +1,24 @@
-"""Particle history containers -- the part of ``particles/smoothing.py`` that touches the
-step loop (``hist.save(smc)``, core.py:362-363; classes at smoothing.py:151-270).  The off-line
-smoothing algorithms that consume a history are outside the accelerated path.
+"""Particle history containers (``hist.save(smc)``, core.py:362-363; classes at smoothing.py:151-270) and the
+off-line FFBS smoothers of ``ParticleHistory`` (smoothing.py:278-423) on the device.
 
 The reference stores references to ``smc.X / A / wgts`` (it allocates new arrays every step).
 The device loop ping-pongs two buffers instead, so a history OWNS what it saves: ``save`` clones
 the device arrays (8(d+2) bytes per particle per saved step -- at N = 1e7 keep the window short).
+
+Backward sampling (``backward_sampling_ON2 / _mcmc / _reject``): when the transition density is a stock model's
+``PX`` (``state_space_models.transition_spec``) the whole backward pass is ONE kernel launch
+(csrc/smcb_smooth.cu); otherwise the same algorithms run with ``fk.logpt`` called on CUDA tensors, with the
+library's sampling, CDF and gather kernels underneath.  There is no CPU path.
 """
+import ctypes as C
 from collections import deque
 
+import numpy as np
 import torch
 
+from . import _lib
 from . import resampling as rs
+from .device import as_device, context, ptr
 
 
 def _own(x):
@@ -97,3 +105,209 @@ class ParticleHistory(RollingParticleHistory):
                 n = int(self.A[t + 1][n])
             traj.append(self.X[t][n])
         return traj[::-1]
+
+    # ------------------------------------------------------------------ FFBS
+    # Extra keyword arguments of the samplers (optional, as SMC(seed=, noise=)): ``seed`` re-keys the device
+    # generator first; ``noise`` is a dict of injected randomness for parity tests -- ``idx_T`` (M,) int, the
+    # final-time indices, and per method:
+    #   ON2     u (M, T-1): the uniform of the draw of trajectory m at time t;
+    #   MCMC    prop (T-1, nsteps, M) int, lu (T-1, nsteps, M): proposals and log-uniforms of each step;
+    #   reject  prop (T-1, M, max_trials) int, lu (T-1, M, max_trials): the trial-th proposal / log-uniform of
+    #           trajectory m, and u_exact (T-1, M): the uniform of its exact fallback draw.
+    def _init_backward_sampling(self, M, noise=None):
+        """smoothing.py:278-281: idx (T, M) int64 on the device, idx[T-1] = multinomial(W_{T-1}, M)."""
+        dev = self.X[-1].device
+        idx = torch.empty((self.T, M), dtype=torch.int64, device=dev)
+        if noise is not None and noise.get("idx_T") is not None:
+            idx[-1] = as_device(noise["idx_T"], dtype=torch.int64, device=dev)
+        else:
+            idx[-1] = rs.multinomial(self.wgts[-1].W, M=M)
+        return idx
+
+    def _output_backward_sampling(self, paths):
+        """smoothing.py:283-289: a list of T views of ONE (T, M[, d]) tensor; squeezed when M = 1."""
+        if paths.shape[1] == 1:
+            paths = paths[:, 0]
+        return [paths[t] for t in range(self.T)]
+
+    def backward_sampling_ON2(self, M, seed=None, noise=None):
+        """O(N^2) FFBS, smoothing.py:291-311: paths[t][m] is component t of trajectory m."""
+        return self._backward(_lib.SMOOTH_ON2, int(M), seed, noise)
+
+    def backward_sampling_mcmc(self, M, nsteps=1, seed=None, noise=None):
+        """MCMC backward sampling (independent Metropolis steps with multinomial proposals, started at the
+        genealogy), smoothing.py:313-350; Dau & Chopin (2022)."""
+        return self._backward(_lib.SMOOTH_MCMC, int(M), seed, noise, nsteps=int(nsteps))
+
+    def backward_sampling_reject(self, M, max_trials=None, seed=None, noise=None):
+        """Hybrid rejection backward sampling, smoothing.py:352-423: at most ``max_trials`` (default M) proposals
+        per trajectory and time, then the exact O(N) draw.  Needs ``fk.upper_bound_trans``; sets ``acc_rate``,
+        (T-1,) = (M - nrejected) / nprops per t."""
+        M = int(M)
+        max_trials = M if max_trials is None else int(max_trials)
+        bounds = np.array([self.fk.upper_bound_trans(t + 1) for t in range(self.T - 1)], dtype=np.float64)
+        return self._backward(_lib.SMOOTH_REJECT, M, seed, noise, max_trials=max_trials, bounds=bounds)
+
+    def backward_sampling_qmc(self, M):
+        raise NotImplementedError("QMC backward sampling needs SQMC (qmc=True), which is outside the "
+                                  "accelerated path")
+
+    def two_filter_smoothing(self, *args, **kwargs):
+        raise NotImplementedError("two-filter smoothing is not built in particles_b200")
+
+    # -------------------------------------------------------------- plumbing
+    def _history_desc(self, method, M):
+        """Descriptor with the per-t pointer tables of the history, and the tensors it points into."""
+        Xs = [as_device(x) if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float64) else x
+              for x in self.X]
+        shape = tuple(Xs[0].shape)
+        if any(tuple(x.shape) != shape for x in Xs):
+            raise ValueError("backward sampling: the particle arrays differ in shape over time")
+        strides = {tuple(x.stride()) for x in Xs}
+        if len(strides) != 1:
+            Xs = [x.contiguous() for x in Xs]
+        d = _lib.SmoothDesc()
+        d.method, d.T, d.N, d.M = method, self.T, shape[0], M
+        d.dim = 1 if len(shape) == 1 else shape[1]
+        st = Xs[0].stride()
+        d.x_stride_n, d.x_stride_c = st[0], (st[1] if len(shape) > 1 else 0)
+        dev = Xs[0].device
+        lws = [w.lw.contiguous() for w in self.wgts]
+        As = list(self.A)
+        keep = {"X": Xs, "lw": lws, "A": As,
+                "tX": torch.tensor([x.data_ptr() for x in Xs], dtype=torch.int64, device=dev),
+                "tlw": torch.tensor([w.data_ptr() for w in lws], dtype=torch.int64, device=dev),
+                "tA": torch.tensor([0 if a is None else a.data_ptr() for a in As], dtype=torch.int64, device=dev)}
+        d.X, d.lw, d.A = keep["tX"].data_ptr(), keep["tlw"].data_ptr(), keep["tA"].data_ptr()
+        return d, keep, Xs
+
+    def _cdfs(self, N, dev):
+        """(T-1, N) inclusive prefix sums of W_t (the one fp64 scratch of the MCMC / reject samplers); rows padded to
+        an even length so that each is 16-byte aligned for smcb_cumsum."""
+        ctx = context(dev)
+        cdf = torch.empty((max(self.T - 1, 1), N + (N & 1)), dtype=torch.float64, device=dev)
+        W = torch.empty(N, dtype=torch.float64, device=dev)
+        for t in range(self.T - 1):
+            w = self.wgts[t]
+            _lib.check(ctx.lib.smcb_weights_from_stats(ctx.handle, ptr(w.lw), N, ptr(w._stats), ptr(W)))
+            _lib.check(ctx.lib.smcb_cumsum(ctx.handle, ptr(W), N, ptr(cdf[t])))
+        return cdf
+
+    def _backward(self, method, M, seed, noise, nsteps=1, max_trials=0, bounds=None):
+        if M < 1:
+            raise ValueError("backward sampling: M must be >= 1")
+        from .state_space_models import transition_spec
+        ctx = context(self.X[-1].device)
+        if seed is not None:
+            ctx.seed(seed)
+        spec = transition_spec(self.fk)
+        idx = self._init_backward_sampling(M, noise)
+        if spec is None:
+            idx = self._plugin(method, M, idx, noise, nsteps, max_trials, bounds)
+        d, keep, Xs = self._history_desc(method if spec is not None else _lib.SMOOTH_GATHER, M)
+        dev = Xs[0].device
+        T, N, D = self.T, d.N, d.dim
+        paths = torch.empty((T, M) + ((D,) if Xs[0].ndim > 1 else ()), dtype=torch.float64, device=dev)
+        d.idx, d.paths = idx.data_ptr(), paths.data_ptr()
+        if spec is not None:
+            d.model, d.n_params = spec["model"], len(spec["params"])
+            for i, v in enumerate(spec["params"]):
+                d.params[i] = float(v)
+            if spec["step_consts"] is not None:
+                keep["sc"] = as_device(spec["step_consts"], device=dev)
+                d.step_consts = keep["sc"].data_ptr()
+            d.idx_T = idx[-1].data_ptr()           # read, then rewritten unchanged, by the same thread
+            d.nsteps, d.max_trials = nsteps, max_trials
+            nz = noise or {}
+            if method == _lib.SMOOTH_ON2 and nz.get("u") is not None:
+                keep["u"] = as_device(np.asarray(nz["u"]).reshape(M, T - 1), device=dev)
+                d.u = keep["u"].data_ptr()
+            if method != _lib.SMOOTH_ON2:
+                if nz.get("prop") is not None:
+                    shape = (T - 1, nsteps, M) if method == _lib.SMOOTH_MCMC else (T - 1, M, max_trials)
+                    keep["prop"] = as_device(np.asarray(nz["prop"]).reshape(shape), dtype=torch.int64, device=dev)
+                    keep["lu"] = as_device(np.asarray(nz["lu"]).reshape(shape), device=dev)
+                    d.prop, d.lu = keep["prop"].data_ptr(), keep["lu"].data_ptr()
+                elif T > 1:
+                    keep["cdf"] = self._cdfs(N, dev)
+                    d.cdf, d.cdf_ld = keep["cdf"].data_ptr(), keep["cdf"].shape[1]
+            if method == _lib.SMOOTH_REJECT:
+                if nz.get("u_exact") is not None:
+                    keep["u_exact"] = as_device(np.asarray(nz["u_exact"]).reshape(T - 1, M), device=dev)
+                    d.u_exact = keep["u_exact"].data_ptr()
+                keep["bounds"] = as_device(bounds if T > 1 else np.zeros(1), device=dev)
+                keep["counts"] = torch.zeros((max(T - 1, 1), 2), dtype=torch.int64, device=dev)
+                d.log_bound, d.counts = keep["bounds"].data_ptr(), keep["counts"].data_ptr()
+        _lib.check(ctx.lib.smcb_backward_sample(ctx.handle, C.byref(d)))
+        if spec is not None and method == _lib.SMOOTH_REJECT:
+            cnt = keep["counts"].cpu().numpy()[: T - 1].astype(np.float64)
+            with np.errstate(divide="ignore", invalid="ignore"):
+                self.acc_rate = cnt[:, 0] / cnt[:, 1]
+        # the pointer tables and scratch may be freed now: the caching allocator hands their memory only to work
+        # enqueued later on this stream.  The (T, M) indices of the last pass stay inspectable.
+        self._bs_idx = idx
+        return self._output_backward_sampling(paths)
+
+    # ----------------------------------------------------------- plugin path
+    def _exact_draw(self, t, xn, u, out):
+        """smoothing.py:310 / 418-421 for one trajectory: searchsorted(cumsum(exp_and_normalise(lw_t +
+        logpt(t + 1, X_t, xn))), u) written into the device int64 scalar ``out``."""
+        ctx = context(out.device)
+        W = rs.exp_and_normalise(self.wgts[t].lw + as_device(self.fk.logpt(t + 1, self.X[t], xn)))
+        cdf = rs.cumsum(W)
+        su = rs._uniforms(1, W) if u is None else torch.full((1,), float(u), dtype=torch.float64, device=W.device)
+        _lib.check(ctx.lib.smcb_searchsorted(ctx.handle, ptr(cdf), W.shape[0], ptr(su), 1, C.c_void_p(out.data_ptr())))
+
+    def _plugin(self, method, M, idx, noise, nsteps, max_trials, bounds):
+        """The reference's loops with ``fk.logpt`` on CUDA tensors (vectorised over M for MCMC / reject, over N per
+        (t, m) for ON2); indices stay on the device."""
+        nz = noise or {}
+        T = self.T
+        dev = idx.device
+        X = self.X
+        if method == _lib.SMOOTH_ON2:
+            u = None if nz.get("u") is None else np.asarray(nz["u"]).reshape(M, T - 1)
+            for m in range(M):
+                for t in reversed(range(T - 1)):
+                    xn = X[t + 1][idx[t + 1, m]]
+                    self._exact_draw(t, xn, None if u is None else u[m, t], idx[t, m])
+            return idx
+        if method == _lib.SMOOTH_MCMC:
+            prop_in = None if nz.get("prop") is None else as_device(np.asarray(nz["prop"]).reshape(T - 1, nsteps, M),
+                                                                     dtype=torch.int64, device=dev)
+            lu_in = None if nz.get("lu") is None else as_device(np.asarray(nz["lu"]).reshape(T - 1, nsteps, M),
+                                                                 device=dev)
+            for t in reversed(range(T - 1)):
+                xn = X[t + 1][idx[t + 1]]
+                idx[t] = self.A[t + 1][idx[t + 1]]
+                for i in range(nsteps):
+                    prop = rs.multinomial_iid(self.wgts[t].W, M=M) if prop_in is None else prop_in[t, i]
+                    lpr = (as_device(self.fk.logpt(t + 1, X[t][prop], xn))
+                           - as_device(self.fk.logpt(t + 1, X[t][idx[t]], xn)))
+                    lu = torch.log(rs._uniforms(M, lpr)) if lu_in is None else lu_in[t, i]
+                    idx[t] = torch.where(lu < lpr, prop, idx[t])
+            return idx
+        prop_in = None if nz.get("prop") is None else as_device(np.asarray(nz["prop"]).reshape(T - 1, M, max_trials),
+                                                                 dtype=torch.int64, device=dev)
+        lu_in = None if nz.get("lu") is None else as_device(np.asarray(nz["lu"]).reshape(T - 1, M, max_trials),
+                                                             device=dev)
+        u_exact = None if nz.get("u_exact") is None else np.asarray(nz["u_exact"]).reshape(T - 1, M)
+        self.acc_rate = np.zeros(T - 1)
+        for t in reversed(range(T - 1)):
+            where = torch.arange(M, device=dev)
+            who = X[t + 1][idx[t + 1]]
+            nprops, ntrials, nrej = 0, 0, M
+            while nrej > 0 and ntrials < max_trials:
+                nprops += nrej
+                prop = rs.multinomial_iid(self.wgts[t].W, M=nrej) if prop_in is None else prop_in[t, where, ntrials]
+                lpr = as_device(self.fk.logpt(t + 1, X[t][prop], who)) - float(bounds[t])
+                lu = torch.log(rs._uniforms(nrej, lpr)) if lu_in is None else lu_in[t, where, ntrials]
+                ntrials += 1
+                acc = lu < lpr
+                idx[t, where[acc]] = prop[acc]
+                where, who = where[~acc], who[~acc]
+                nrej = int(where.shape[0])
+            for m in where.tolist():
+                self._exact_draw(t, X[t + 1][idx[t + 1, m]], None if u_exact is None else u_exact[t, m], idx[t, m])
+            self.acc_rate[t] = (M - nrej) / nprops if nprops else np.nan
+        return idx

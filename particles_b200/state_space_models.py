@@ -19,6 +19,14 @@ from . import distributions as dists
 from .core import FeynmanKac
 
 
+err_msg_missing_cst = """
+    State-space model %s is missing method upper_bound_log_pt, which provides
+    log of constant C_t, such that
+    p(x_t|x_{t-1}) <= C_t
+    This is required for smoothing algorithms based on rejection
+    """
+
+
 class StateSpaceModel:
     """particles/state_space_models.py:172-296."""
 
@@ -44,6 +52,10 @@ class StateSpaceModel:
 
     def proposal(self, t, xp, data):
         raise NotImplementedError(self._error_msg("proposal"))
+
+    def upper_bound_log_pt(self, t):
+        """state_space_models.py:261-266: log of a constant C_t >= p(x_t | x_{t-1}) (rejection smoothing)."""
+        raise NotImplementedError(err_msg_missing_cst % self.__class__.__name__)
 
     def simulate_given_x(self, x):
         lag_x = [None] + x[:-1]
@@ -80,6 +92,10 @@ class Bootstrap(FeynmanKac):
 
     def logpt(self, t, xp, x):
         return self.ssm.PX(t, xp).logpdf(x)
+
+    def upper_bound_trans(self, t):
+        """state_space_models.py:345-346."""
+        return self.ssm.upper_bound_log_pt(t)
 
 
 class GuidedPF(Bootstrap):
@@ -330,7 +346,7 @@ def spec_discretecox(m, T, data=None):
 
 def spec_bearings(m, T):
     x0 = np.asarray(m.x0, dtype=np.float64).reshape(4)
-    p = [m.sigmaX, m.sigmaY, np.log(m.sigmaY)] + list(x0)
+    p = [m.sigmaX, m.sigmaY, np.log(m.sigmaY)] + list(x0) + [np.log(m.sigmaX)]
     return {"model": _lib.MODEL_BEARINGS, "params": p, "dim": 4, "dy": 1, "n_noise": 2, "proposal": False}
 
 
@@ -406,3 +422,39 @@ def fused_spec(fk):
     spec["fk"] = kind
     spec["data"] = _flat_data(fk.data, spec.get("dy", 1))
     return spec
+
+
+def _defining_class(cls, name):
+    return next((c for c in cls.__mro__ if name in c.__dict__), None)
+
+
+def transition_spec(fk):
+    """Return the device description of ``fk.logpt(t, xp, x) = PX(t, xp).logpdf(x)`` (backward sampling,
+    csrc/smcb_smooth.cu) or None if the density must be evaluated by calling ``fk.logpt``.
+
+    Wider than ``fused_spec``: smoothing users subclass a stock model to add ``upper_bound_log_pt`` or
+    ``add_func`` (the reference's book scripts do), so the model is accepted when the class that DEFINES ``PX`` in
+    its MRO is a stock class, and the Feynman-Kac object's ``logpt`` is ``Bootstrap.logpt`` (ours or the
+    reference's, inherited by every Feynman-Kac kind).  Keys: model, params, dim, step_consts (or None)."""
+    owner = _defining_class(type(fk), "logpt")
+    if owner is None or owner.__name__ != "Bootstrap" or owner.__module__ not in _TRUSTED_MODULES:
+        return None
+    ssm = getattr(fk, "ssm", None)
+    px = None if ssm is None else _defining_class(type(ssm), "PX")
+    if px is None or px.__module__ not in _TRUSTED_MODULES:
+        return None
+    make = _SPECS.get(px.__name__)
+    if make is None:
+        return None
+    data = getattr(fk, "data", None)
+    T = 0 if data is None else len(data)
+    if make is spec_discretecox:        # its step constants describe the observations, not PX: none needed here
+        spec = make(ssm, T, [np.zeros(1)] * max(T, 1))
+    elif make is spec_mvlingauss:
+        spec = make(ssm, T, None)
+    else:
+        spec = make(ssm, T)
+    if spec is None:
+        return None
+    return {"model": spec["model"], "params": list(spec["params"]), "dim": int(spec.get("dim", 1)),
+            "step_consts": spec.get("step_consts") if make is spec_gordon else None}
