@@ -282,6 +282,10 @@ int smcb_filter_step_timed(smcb_filter *f, int64_t nsteps, double *out8);
  * out[0]=t, [1]=cur buffer index, [2]=rs_flag of last step, [3]=logLt, [4]=ESS,
  * [5]=log_mean_w, [6]=max lw, [7]=sum w */
 int smcb_filter_state(smcb_filter *f, double *out8);
+/* fused pairs of streaming steps (env SMCB_FUSE, read at smcb_filter_create: 0 off, 1 on, 2 fuse whenever
+ * allowed): out[0] = launches that ran their step and the next one, out[1] = launches whose step was already
+ * done (no-op), out[2] = launches whose pre-computed step resampled after all (misprediction).  Synchronises. */
+int smcb_filter_fusion_stats(smcb_filter *f, int64_t *out3);
 
 /* ---------------------------------------------------------------------------
  * off-line smoothing: FFBS backward sampling over a stored history (particles/smoothing.py:278-423)

@@ -108,6 +108,7 @@ PROTOTYPES = {
     "smcb_p2p_free": (C.c_int, [C.c_void_p]),
     "smcb_filter_step_timed": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_double)]),
     "smcb_filter_state": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),
+    "smcb_filter_fusion_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "smcb_backward_sample": (C.c_int, [C.c_void_p, C.POINTER(SmoothDesc)]),
 }
 

@@ -66,6 +66,32 @@ def _is_apf(fk):
     return fk.isAPF if hasattr(fk, "isAPF") else ("logeta" in dir(fk))
 
 
+def fusion_schedule(summaries, N, ESSrmin, mode, batches):
+    """What each step-kernel launch of a 1-D single-device fused filter did, replayed on the host from its (T, 4)
+    summary table: a list with one entry per step t >= 1, "resample", "plain" (streaming step), "fused" (streaming
+    step t and step t + 1), "noop" (step t done by launch t - 1) or "mispredicted" (step t done by launch t - 1,
+    then resampled after all).  ``batches`` lists the step counts of the ``step()`` calls; ``mode`` is SMCB_FUSE.
+    The predictor is the kernel's: fuse when 2 ESS_{t-1} - ESS_{t-2} >= N * ESSrmin (ESS_{t-1} alone at t = 1)."""
+    table = np.asarray(summaries)
+    T = table.shape[0]
+    ess, rs_ = table[:, 0], table[:, 2] != 0
+    kinds, pre, end = [], -1, 0
+    for b in batches:
+        start, end = end, end + int(b)
+        for t in range(max(start, 1), end):
+            if pre == t:
+                kinds.append("mispredicted" if rs_[t] else "noop")
+            elif rs_[t]:
+                kinds.append("resample")
+            elif mode and t + 1 < T and t + 1 < end and (
+                    mode == 2 or 2.0 * ess[t - 1] - (ess[t - 2] if t >= 2 else ess[t - 1]) >= float(N) * ESSrmin):
+                kinds.append("fused")
+                pre = t + 1
+            else:
+                kinds.append("plain")
+    return kinds
+
+
 class _FusedEngine:
     """Owns the device buffers of one fused filter and the smcb_filter handle."""
 
@@ -174,6 +200,13 @@ class _FusedEngine:
         out = (C.c_double * 8)()
         _lib.check(self.lib.smcb_filter_state(self.handle, out))
         return list(out)
+
+    def fusion_stats(self):
+        """Counts of the fused pairs of streaming steps (SMCB_FUSE): launches that ran two steps, launches that
+        found their step done, and launches whose pre-computed step resampled after all."""
+        out = (C.c_int64 * 3)()
+        _lib.check(self.lib.smcb_filter_fusion_stats(self.handle, out))
+        return dict(zip(("fused", "noop", "mispredicted"), (int(v) for v in out)))
 
     def close(self):
         """Free the filter handle.  Peer-mapped memory (mailboxes, arenas) belongs to the per-(process, group)

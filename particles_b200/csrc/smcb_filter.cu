@@ -62,19 +62,8 @@ static int filter_setup(smcb_filter *f, smcb_ctx *c, const smcb_filter_desc *d) 
     if (rc) return rc;
 
     const int64_t n = d->n;
-    constexpr size_t kHdr = 512;       // StepState[2] | grid-barrier counter | timeout flag
-    static_assert(2 * sizeof(StepState) <= 384, "StepState outgrew its header slot");
-    const size_t part = (size_t)2 * kMaxStepGrid * kPartStride * sizeof(double);
-    const size_t agg = (size_t)(kMaxStepGrid + 8) * sizeof(double);
-    SMCB_CUDA(cudaMalloc(&f->mem, kHdr + part + agg));
-    SMCB_CUDA(cudaMemsetAsync(f->mem, 0, kHdr + part + agg, c->stream));
     FilterArgs &a = f->args;
     memset(&a, 0, sizeof(a));
-    a.st = reinterpret_cast<StepState *>(f->mem);
-    a.bar = reinterpret_cast<unsigned long long *>(f->mem + 384);
-    a.sync_timeout = reinterpret_cast<int *>(f->mem + 392);
-    a.partials = reinterpret_cast<double *>(f->mem + kHdr);
-    a.blk_agg = reinterpret_cast<double *>(f->mem + kHdr + part);
     a.math_tab = c->math_tab;
     a.X[0] = d->X[0]; a.X[1] = d->X[1]; a.lw[0] = d->lw[0]; a.lw[1] = d->lw[1];
     a.A = reinterpret_cast<long long *>(d->A);
@@ -127,6 +116,29 @@ static int filter_setup(smcb_filter *f, smcb_ctx *c, const smcb_filter_desc *d) 
     }
     a.world = d->world > 1 ? d->world : 1;
     a.rank = d->world > 1 ? d->rank : 0;
+    // fused pairs of streaming steps (smcb_step.cuh): 1-D, single device; SMCB_FUSE=0 off, 1 on (default),
+    // 2 fuse whenever allowed (no predictor: every resampling step after a streaming one is a misprediction)
+    {
+        const char *v = getenv("SMCB_FUSE");
+        const int mode = (!v || !*v) ? 1 : (v[0] == '0' ? 0 : (v[0] == '2' ? 2 : 1));
+        a.fuse_mode = (d->dim == 1 && a.world == 1) ? mode : 0;
+    }
+    // device memory: header (StepState[2] | fusion words | grid-barrier counter | timeout flag) + partials + block
+    // aggregates [+ the second step's slab records of a fused pair]
+    constexpr size_t kHdr = 512;
+    static_assert(2 * sizeof(StepState) <= 256, "StepState outgrew its header slot");
+    const size_t part = (size_t)kPartSlots * kMaxStepGrid * kPartStride * sizeof(double);
+    const size_t agg = (size_t)(kMaxStepGrid + 8) * sizeof(double);
+    const size_t slab = a.fuse_mode ? (size_t)f->grid_move * f->slab_doubles * sizeof(double) : 0;
+    SMCB_CUDA(cudaMalloc(&f->mem, kHdr + part + agg + slab));
+    SMCB_CUDA(cudaMemsetAsync(f->mem, 0, kHdr + part + agg, c->stream));
+    a.st = reinterpret_cast<StepState *>(f->mem);
+    a.fuse = reinterpret_cast<long long *>(f->mem + 256);
+    a.bar = reinterpret_cast<unsigned long long *>(f->mem + 384);
+    a.sync_timeout = reinterpret_cast<int *>(f->mem + 392);
+    a.partials = reinterpret_cast<double *>(f->mem + kHdr);
+    a.blk_agg = reinterpret_cast<double *>(f->mem + kHdr + part);
+    a.fuse_slab = a.fuse_mode ? reinterpret_cast<double *>(f->mem + kHdr + part + agg) : nullptr;
     a.local_stats = d->local_stats;
     a.gathered = d->gathered;
     a.mail_local = (a.world > 1) ? d->mail_local : nullptr;
@@ -191,6 +203,7 @@ static int launch_one(smcb_filter *f) {
 extern "C" int smcb_filter_step_local(smcb_filter *f) {
     SMCB_REQUIRE(f != nullptr && f->args.world > 1 && f->args.mail_local == nullptr,
                  "smcb_filter_step_local: not a sharded filter with the host-driven exchange");
+    f->args.batch_end = f->t_host + 1;
     int rc = launch_one(f);
     if (rc) return rc;
     return f->launch_publish(f);
@@ -206,6 +219,7 @@ extern "C" int smcb_filter_step(smcb_filter *f, int64_t nsteps) {
     SMCB_REQUIRE(f->args.world == 1 || f->args.mail_local != nullptr,
                  "smcb_filter_step: sharded filters without a peer mailbox use step_local / step_finish");
     if (nsteps <= 0) return SMCB_OK;
+    f->args.batch_end = f->t_host + nsteps;       // a fused pair never reaches past the steps asked for
     // the device needs no host decision between steps: enqueue them all, then the tail that finalises the last
     for (int64_t i = 0; i < nsteps; i++) {
         int rc = launch_one(f);
@@ -239,6 +253,7 @@ extern "C" int smcb_filter_step_timed(smcb_filter *f, int64_t nsteps, double *ou
         if (e != cudaSuccess) { fail(e, "cudaEventCreate"); break; }
     }
     f->timed = true;
+    f->args.batch_end = t_first + nsteps;
     for (int64_t i = 0; rc == SMCB_OK && i <= nsteps; i++) {
         cudaEventRecord(ev[2 * i], s);
         rc = (i < nsteps) ? launch_one(f) : f->launch_tail(f);
@@ -295,6 +310,15 @@ extern "C" int smcb_filter_state(smcb_filter *f, double *out8) {
                   (long long)s.t, (long long)(f->t_host - 1));
         return SMCB_ECUDA;
     }
+    return SMCB_OK;
+}
+
+extern "C" int smcb_filter_fusion_stats(smcb_filter *f, int64_t *out3) {
+    SMCB_REQUIRE(f && out3, "smcb_filter_fusion_stats: NULL argument");
+    long long h[4];
+    SMCB_CUDA(cudaMemcpyAsync(h, f->args.fuse, sizeof(h), cudaMemcpyDeviceToHost, f->ctx->stream));
+    SMCB_CUDA(cudaStreamSynchronize(f->ctx->stream));
+    for (int i = 0; i < 3; i++) out3[i] = h[1 + i];
     return SMCB_OK;
 }
 

@@ -12,14 +12,21 @@
 //     resampling:     W_i = exp(lw_i - m)/s -> CDF of the CTA's own range (16 B/particle)
 //                     -> grid barrier -> su_k -> A_k = search(cdf) -> xp = X[A_k] -> x' -> lw' = logG
 //                     -> partials                                                         40 B/particle
+//     fused pair (1-D, one device): a streaming step t whose successor is predicted not to resample also runs
+//                     step t+1 while the particle sits in registers: x_{t-1}, lw_{t-1} in once, x_t, lw_t out to
+//                     buffers t & 1, x_{t+1}, lw_{t+1} out to buffers (t+1) & 1 in place       24 B/particle/step
+//                     Launch t+1 then only runs its prologue; if that says "resample", it overwrites the
+//                     speculative step t+1 from the intact buffers t & 1.
 //   k_tail(t)  (one CTA, once per enqueued batch): the prologue alone, so that the summaries of the last
 //              enqueued step exist before the host reads them.  Idempotent with the next k_step.
 //
 // The step index is a kernel argument (the host mirrors it); everything else a step needs from its
-// predecessor is in the partials (double-buffered by step parity) and in S_{t-2}.
+// predecessor is in the partials (four rows per CTA, indexed by step mod 4: a fused launch reads those of t-1 and
+// writes those of t and t+1) and in S_{t-2}.
 #include <string.h>
 
 #include <new>
+#include <type_traits>
 
 #include "smcb_common.cuh"
 #include "smcb_math.cuh"
@@ -38,6 +45,7 @@ constexpr int kMailScan = 17;       // slot[17] = t + 1 once the sender's CDF of
 constexpr int kMaxStepGrid = 256;   // CTAs of the step kernel: ONE per SM (132 on an H100), each owning a contiguous range
 constexpr int kMaxD = 4;
 constexpr int kTailBlock = 256;     // threads of the one-CTA helper kernels (>= kMaxStepGrid: one partial row per thread)
+constexpr int kPartSlots = 4;       // partial rows per CTA: step s uses row s % 4
 #ifndef SMCB_SPECULATE
 #define SMCB_SPECULATE 1         // sharded filters: start the streaming pass before the peers' statistics arrive
 #endif
@@ -84,7 +92,13 @@ struct FilterArgs {
     const double *z_in, *u_in;
     StepState *st;           // [2]
     int *sync_timeout;       // a bounded wait expired (diagnostic; results are then invalid)
-    double *partials;        // [2][kMaxStepGrid][kPartStride]
+    double *partials;        // [kPartSlots][kMaxStepGrid][kPartStride]
+    // fused pairs of streaming steps (1-D, single device)
+    int fuse_mode;           // 0 off, 1 on with the predictor, 2 fuse whenever allowed (SMCB_FUSE)
+    int64_t batch_end;       // first step the host has not enqueued yet: step t+1 is only fused below it
+    long long *fuse;         // [0] the step the previous launch pre-computed; [1..3] fused pairs, no-op launches,
+                             // mispredicted launches (pre-computed step that resampled after all)
+    double *fuse_slab;       // grid x StepCfg::kSlabDoubles: the slab records of the second step of a pair
     unsigned long long *bar; // grid-barrier arrivals, never reset
     double *blk_agg;         // multinomial: per-CTA sums of the exponential spacings (grid + 1)
     const double *math_tab;  // smcb_tables.h, built at context creation
@@ -380,7 +394,7 @@ __device__ __forceinline__ void write_partial(const FilterArgs &a, long long t, 
         v[0] = w4[0]; v[1] = w4[1]; v[2] = w4[2]; v[3] = w4[3];
     }
     if (threadIdx.x == 0) {
-        double *p = a.partials + ((size_t)(t & 1) * kMaxStepGrid + blockIdx.x) * kPartStride;
+        double *p = a.partials + ((size_t)(t % kPartSlots) * kMaxStepGrid + blockIdx.x) * kPartStride;
         p[0] = mx[0]; p[1] = v[0]; p[2] = v[1]; p[3] = 0.0;
         p[4] = APF ? mx[1] : mx[0]; p[5] = APF ? v[2] : v[0]; p[6] = APF ? v[3] : v[1]; p[7] = 0.0;
 #pragma unroll
@@ -416,7 +430,7 @@ template <bool APF>
 __device__ __forceinline__ void shard_totals(const FilterArgs &a, long long s, bool mom, StepSmem &sh, double (&loc)[16]) {
     const int G = a.grid, tid = threadIdx.x;
     if (tid < 32) {
-        const double *base = a.partials + (size_t)(s & 1) * kMaxStepGrid * kPartStride;
+        const double *base = a.partials + (size_t)(s % kPartSlots) * kMaxStepGrid * kPartStride;
         constexpr int kR = kMaxStepGrid / 32;
         double pm[kR], ps[kR], pq[kR], xm[kR], xs[kR], xq[kR];
         double mw = -CUDART_INF, ma = -CUDART_INF;
@@ -502,6 +516,7 @@ struct StepDecision {
     double reset_c;           // log-weight every resampled particle restarts from (minus logeta[A] for an APF)
     double xm, xs;            // (max, sum exp) of this shard's (auxiliary) weights: the CDF's normalisation
     double p_b, p_next;       // this CTA's range of the CDF
+    double ess;               // ESS of step t - 1 (the fused-pair predictor)
 };
 
 // compute_summaries of step s = t - 1 (core.py:351-367) + time_to_resample of step t (core.py:181-183),
@@ -625,6 +640,7 @@ __device__ __forceinline__ StepDecision prologue_end(const FilterArgs &a, long l
     d.reset_c = rc;
     d.xm = xl.m; d.xs = xl.s;
     d.p_b = 0.0; d.p_next = 0.0;
+    d.ess = ess;
     if (writer && tid == 0) {
         double *row = a.summaries + (size_t)s * SMCB_SUMMARY_STRIDE;
         row[0] = ess; row[1] = logLt; row[2] = (double)rs_s; row[3] = log_mean;
@@ -648,7 +664,7 @@ __device__ __forceinline__ StepDecision prologue_end(const FilterArgs &a, long l
         // CTA), and the scan needs no look-back at all.
         double v = 0.0;
         if (tid < a.grid) {                      // row tid of the partials: this CTA's (auxiliary) weight mass
-            const double *row = a.partials + ((size_t)(s & 1) * kMaxStepGrid + tid) * kPartStride + (APF ? 4 : 0);
+            const double *row = a.partials + ((size_t)(s % kPartSlots) * kMaxStepGrid + tid) * kPartStride + (APF ? 4 : 0);
             v = __ldcg(row + 1) * shift_factor(__ldcg(row), d.xm) / d.xs;
         }
         cta_prefix<BS>(v, sh, d.p_b, d.p_next);
@@ -1085,6 +1101,26 @@ __device__ __forceinline__ int shard_of(const double *goff, const double *gpi, i
     return k;
 }
 
+// what one step of the streaming pass needs besides the particles, and where it writes them
+struct StepIo {
+    long long t;
+    StepK k;
+    const double *zin;       // injected normals of step t, (NZ, n), or NULL
+    double *Xo, *lwo;        // buffers [t & 1]
+    bool last_apf;           // step t + 1 exists (an APF computes its auxiliary weights)
+};
+
+__device__ __forceinline__ StepIo step_io(const FilterArgs &a, long long t, int nz) {
+    StepIo io;
+    io.t = t;
+    io.k = step_consts(a, t);
+    io.zin = a.z_in ? a.z_in + (size_t)t * nz * a.n : nullptr;
+    io.Xo = a.X[t & 1];
+    io.lwo = a.lw[t & 1];
+    io.last_apf = t + 1 < a.T;
+    return io;
+}
+
 // ---------------------------------------------------------------------------
 // the step kernel: resample_move + reweight_particles (+ compute_summaries of the previous step)
 // (core.py:323-367)
@@ -1120,22 +1156,41 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
     const bool speculate = SMCB_SPECULATE && a.world > 1 && a.mail_local != nullptr && !a.rs_global && !pred_rs;
     StepDecision dec;
     dec.rs = 0; dec.nrs_prev = 0; dec.reset_c = 0.0; dec.xm = 0.0; dec.xs = 1.0; dec.p_b = 0.0; dec.p_next = 0.0;
+    dec.ess = 0.0;
     if (!speculate) dec = prologue_end<APF, BS>(a, t, sh, blockIdx.x == 0, true, pc);
     // (no block barrier on the speculative path: CTA 0's sending lanes sit in their system-scope fence for a few
     // microseconds, and the other warps of that CTA start on the slabs meanwhile -- the dynamic slab schedule absorbs it)
     mbar_wait(&s_tabbar, 0);                           // (the prologue's barriers made the init visible)
     const int cur = (int)((t - 1) & 1);                // step s writes buffers [s & 1]
     const bool rs = dec.rs != 0;                       // (a speculative step enters the resampling branch from below)
+    if (a.fuse_mode != 0 && __ldcg(a.fuse) == t) {
+        // the previous launch ran this step as the second half of a fused pair.  Its x_t, lw_t and partial rows
+        // are in place unless step t resamples after all: then the resampling branch below overwrites them from
+        // buffers [(t-1) & 1], which the fused pass left intact.
+        if (blockIdx.x == 0 && threadIdx.x == 0) a.fuse[rs ? 3 : 2] += 1;
+        if (!rs) return;
+    }
+    // Fuse step t + 1 into this streaming pass?  Only if the host has enqueued it in this batch (a caller that stops
+    // after step t reads Xp from buffers [(t-1) & 1]), and -- a step t + 1 that resamples discards the speculative
+    // half -- if the ESS extrapolated from steps t - 2 and t - 1 stays above the threshold.  Every CTA decides
+    // alike (the prologue's ESS has the same bits everywhere); the choice changes the speed, never the results.
+    bool fuse = false;
+    if (D == 1 && !rs && a.fuse_mode != 0 && a.world == 1 && t + 1 < a.T && t + 1 < a.batch_end) {
+        const double ess2 = (t >= 2) ? __ldcg(&a.st[(t - 2) & 1].ess) : dec.ess;
+        fuse = a.fuse_mode == 2 || 2.0 * dec.ess - ess2 >= (double)a.n_global * a.essrmin;
+    }
+    if (fuse && blockIdx.x == 0 && threadIdx.x == 0) { a.fuse[0] = t + 1; a.fuse[1] += 1; }
     double reset_c = dec.reset_c;
-    const StepK k = step_consts(a, t);
+    const StepIo io0 = step_io(a, t, NZ);
+    const StepK &k = io0.k;
     const StepK kprev = step_consts(a, t - 1);
     const double *__restrict__ Xi = a.X[cur];
     const double *__restrict__ lwi = a.lw[cur];
-    double *__restrict__ Xo = a.X[cur ^ 1];
-    double *__restrict__ lwo = a.lw[cur ^ 1];
+    double *__restrict__ Xo = io0.Xo;
+    double *__restrict__ lwo = io0.lwo;
     const int64_t n = a.n;
-    const double *zin = a.z_in ? a.z_in + (size_t)t * NZ * n : nullptr;
-    const bool last_apf = APF && (t + 1 < a.T);
+    const double *zin = io0.zin;
+    const bool last_apf = APF && io0.last_apf;
     const bool mom = a.moments != nullptr;
     const bool vec_x = (D == 1) || ((n & 1) == 0);     // SoA component rows are 16-byte aligned
     int64_t pstart, pend;
@@ -1146,42 +1201,42 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
     Lse3 aux = lse3_empty();
     int n_slab = 0;                                    // slab records of the streaming branch
 
-    // propagate + reweight one pair of particles; writes x', lw'; returns x', lw' (and the auxiliary
+    // propagate + reweight one pair of particles by step io.t; writes x', lw'; returns x', lw' (and the auxiliary
     // log-weights of the next step for an APF), -inf in masked slots
-    auto do_pair = [&](int64_t p, const double (&xp)[2][D], const double (&base)[2], double (&x)[2][D], double *l,
-                       double *av) {
+    auto do_pair = [&](const StepIo &io, int64_t p, const double (&xp)[2][D], const double (&base)[2],
+                       double (&x)[2][D], double *l, double *av) {
         double z[2][NZ];
 #pragma unroll
         for (int c = 0; c < NZ; c++) {
-            if (zin) {                                   // injected normals: (T, NZ, n)
-                const double *zz = zin + (size_t)c * n;
+            if (io.zin) {                                // injected normals: (T, NZ, n)
+                const double *zz = io.zin + (size_t)c * n;
                 z[0][c] = zz[2 * p];
                 z[1][c] = (2 * p + 1 < n) ? zz[2 * p + 1] : 0.0;
             } else {
-                normal_pair_tab(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t, (uint32_t)c,
+                normal_pair_tab(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)io.t, (uint32_t)c,
                                  z[0][c], z[1][c]);
             }
         }
 #pragma unroll
         for (int j = 0; j < 2; j++) {
             double d;
-            model_move<M, FK>(model, k, xp[j], z[j], x[j], d);
+            model_move<M, FK>(model, io.k, xp[j], z[j], x[j], d);
             l[j] = fix_nan(base[j] + d);                          // Weights.add, resampling.py:241-244
-            if (APF) av[j] = last_apf ? fix_nan(l[j] + model_logeta<M>(model, k, x[j])) : -CUDART_INF;
+            if (APF) av[j] = io.last_apf ? fix_nan(l[j] + model_logeta<M>(model, io.k, x[j])) : -CUDART_INF;
         }
         if (2 * p + 1 < n) {
             if (vec_x) {
 #pragma unroll
-                for (int c = 0; c < D; c++) st2(Xo + (size_t)c * n + 2 * p, x[0][c], x[1][c]);
+                for (int c = 0; c < D; c++) st2(io.Xo + (size_t)c * n + 2 * p, x[0][c], x[1][c]);
             } else {
 #pragma unroll
-                for (int c = 0; c < D; c++) { Xo[(size_t)c * n + 2 * p] = x[0][c]; Xo[(size_t)c * n + 2 * p + 1] = x[1][c]; }
+                for (int c = 0; c < D; c++) { io.Xo[(size_t)c * n + 2 * p] = x[0][c]; io.Xo[(size_t)c * n + 2 * p + 1] = x[1][c]; }
             }
-            st2(lwo + 2 * p, l[0], l[1]);
+            st2(io.lwo + 2 * p, l[0], l[1]);
         } else {
 #pragma unroll
-            for (int c = 0; c < D; c++) { Xo[(size_t)c * n + 2 * p] = x[0][c]; x[1][c] = 0.0; }
-            lwo[2 * p] = l[0];
+            for (int c = 0; c < D; c++) { io.Xo[(size_t)c * n + 2 * p] = x[0][c]; x[1][c] = 0.0; }
+            io.lwo[2 * p] = l[0];
             l[1] = -CUDART_INF;
             if (APF) av[1] = -CUDART_INF;
         }
@@ -1202,27 +1257,26 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
         const bool fast_ok = (zin == nullptr) && vec_x;
         const double *__restrict__ lwi_c = lwi + 2 * pstart;
         const double *__restrict__ Xi_c = Xi + 2 * pstart;
-        double *__restrict__ lwo_c = lwo + 2 * pstart;
-        double *__restrict__ Xo_c = Xo + 2 * pstart;
         const uint64_t gpair0 = (uint64_t)((a.index_offset >> 1) + pstart);
         // one iteration: pairs (relative to pstart) i * kIt + u * 32 + lane.  Loads and arithmetic are separate so
         // that the inputs of the NEXT iteration can be requested before the current one is computed.
         struct In { double base[kU][2]; double xp[kU][2][D]; };
-        auto load_full = [&](int i, In &in) {
+        auto load_full = [&](const double *Xs_c, const double *lws_c, int i, In &in) {
 #pragma unroll
             for (int u = 0; u < kU; u++) {
                 const int o2 = 2 * (i * kIt + u * 32 + lane);
-                const double2 tl = ld2(lwi_c + o2);
+                const double2 tl = ld2(lws_c + o2);
                 in.base[u][0] = tl.x; in.base[u][1] = tl.y;
 #pragma unroll
                 for (int c = 0; c < D; c++) {
-                    const double2 tx = ld2(Xi_c + (size_t)c * n + o2);
+                    const double2 tx = ld2(Xs_c + (size_t)c * n + o2);
                     in.xp[u][0][c] = tx.x; in.xp[u][1][c] = tx.y;
                 }
             }
         };
-        auto compute_full = [&](int i, const In &in, Acc<D> &ac, Lse3 &ax) {
-            double l[2 * kU], av[APF ? 2 * kU : 1], x[2 * kU][D];
+        auto compute_full = [&](const StepIo &io, int i, const In &in, Acc<D> &ac, Lse3 &ax, double (&l)[2 * kU],
+                                double (&x)[2 * kU][D]) {
+            double av[APF ? 2 * kU : 1];
             bool odd = false;                                 // some value is +-inf / NaN (integer test)
 #pragma unroll
             for (int u = 0; u < kU; u++) {
@@ -1230,16 +1284,16 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
                 double z[2][NZ];
 #pragma unroll
                 for (int c = 0; c < NZ; c++)
-                    normal_pair_tab(a.key, gpair0 + (uint64_t)prel, (uint32_t)t, (uint32_t)c, z[0][c], z[1][c]);
+                    normal_pair_tab(a.key, gpair0 + (uint64_t)prel, (uint32_t)io.t, (uint32_t)c, z[0][c], z[1][c]);
 #pragma unroll
                 for (int j2 = 0; j2 < 2; j2++) {
                     double d;
-                    model_move<M, FK>(model, k, in.xp[u][j2], z[j2], x[2 * u + j2], d);
+                    model_move<M, FK>(model, io.k, in.xp[u][j2], z[j2], x[2 * u + j2], d);
                     l[2 * u + j2] = in.base[u][j2] + d;                   // Weights.add, resampling.py:241-244
                     odd |= nonfinite(l[2 * u + j2]);
                     if (APF) {
-                        av[APF ? 2 * u + j2 : 0] = last_apf ? l[2 * u + j2] + model_logeta<M>(model, k, x[2 * u + j2])
-                                                            : -CUDART_INF;
+                        av[APF ? 2 * u + j2 : 0] = io.last_apf ? l[2 * u + j2] + model_logeta<M>(model, io.k, x[2 * u + j2])
+                                                               : -CUDART_INF;
                         odd |= nonfinite(av[APF ? 2 * u + j2 : 0]);
                     }
                 }
@@ -1251,6 +1305,8 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
                     if (APF) av[APF ? q : 0] = fix_nan(av[APF ? q : 0]);
                 }
             }
+            double *const lwo_c = io.lwo + 2 * pstart;
+            double *const Xo_c = io.Xo + 2 * pstart;
 #pragma unroll
             for (int u = 0; u < kU; u++) {
                 const int o2 = 2 * (i * kIt + u * 32 + lane);
@@ -1265,43 +1321,40 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
             }
             if (APF) lse3_add_batch<(APF ? 2 * kU : 1)>(ax, av);
         };
-        auto iteration = [&](int i, Acc<D> &ac, Lse3 &ax) {
-            double l[2 * kU], av[APF ? 2 * kU : 1], x[2 * kU][D];
-            if (fast_ok && i < n_full) {
-                In in;
-                load_full(i, in);
-                compute_full(i, in, ac, ax);
-                return;
-            }
-            // general path: ragged end of the range, the odd last particle, injected normals, odd SoA stride
-            double xp[kU][2][D], base[kU][2];
+        // general path: ragged end of the range, the odd last particle, injected normals, odd SoA stride
+        auto load_general = [&](const double *Xs, const double *lws, int i, In &in) {
             const int64_t qbase = pstart + (int64_t)i * kIt;
 #pragma unroll
             for (int u = 0; u < kU; u++) {
                 const int64_t p = qbase + u * 32 + lane;
                 if (p < pend && 2 * p + 1 < n) {
-                    double2 tl = ld2(lwi + 2 * p);
-                    base[u][0] = tl.x; base[u][1] = tl.y;
+                    double2 tl = ld2(lws + 2 * p);
+                    in.base[u][0] = tl.x; in.base[u][1] = tl.y;
 #pragma unroll
                     for (int c = 0; c < D; c++) {
                         if (vec_x) {
-                            double2 tx = ld2(Xi + (size_t)c * n + 2 * p);
-                            xp[u][0][c] = tx.x; xp[u][1][c] = tx.y;
+                            double2 tx = ld2(Xs + (size_t)c * n + 2 * p);
+                            in.xp[u][0][c] = tx.x; in.xp[u][1][c] = tx.y;
                         } else {
-                            xp[u][0][c] = Xi[(size_t)c * n + 2 * p]; xp[u][1][c] = Xi[(size_t)c * n + 2 * p + 1];
+                            in.xp[u][0][c] = Xs[(size_t)c * n + 2 * p]; in.xp[u][1][c] = Xs[(size_t)c * n + 2 * p + 1];
                         }
                     }
                 } else if (p < pend) {
-                    base[u][0] = lwi[2 * p]; base[u][1] = 0.0;
+                    in.base[u][0] = lws[2 * p]; in.base[u][1] = 0.0;
 #pragma unroll
-                    for (int c = 0; c < D; c++) { xp[u][0][c] = Xi[(size_t)c * n + 2 * p]; xp[u][1][c] = 0.0; }
+                    for (int c = 0; c < D; c++) { in.xp[u][0][c] = Xs[(size_t)c * n + 2 * p]; in.xp[u][1][c] = 0.0; }
                 }
             }
+        };
+        auto compute_general = [&](const StepIo &io, int i, const In &in, Acc<D> &ac, Lse3 &ax, double (&l)[2 * kU],
+                                   double (&x)[2 * kU][D]) {
+            double av[APF ? 2 * kU : 1];
+            const int64_t qbase = pstart + (int64_t)i * kIt;
 #pragma unroll
             for (int u = 0; u < kU; u++) {
                 const int64_t p = qbase + u * 32 + lane;
                 if (p < pend) {
-                    do_pair(p, xp[u], base[u], reinterpret_cast<double (&)[2][D]>(x[2 * u]), l + 2 * u,
+                    do_pair(io, p, in.xp[u], in.base[u], reinterpret_cast<double (&)[2][D]>(x[2 * u]), l + 2 * u,
                             APF ? av + 2 * u : av);
                 } else {
                     l[2 * u] = l[2 * u + 1] = -CUDART_INF;
@@ -1326,7 +1379,6 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
         const int it_small0 = n_iter - n_small;                               // first single-iteration slab
         const int n_big = (it_small0 + slab_it - 1) / slab_it;                // slabs of (up to) slab_it iterations
         n_slab = n_big + n_small;
-        double *s_slab = s_stage;
         const bool lane_rec = a.slab_lane != 0;
         auto grab = [&]() {
             int v = 0;
@@ -1334,39 +1386,93 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
             return __shfl_sync(0xffffffffu, v, 0);
         };
         auto first_it = [&](int sl) { return sl < n_big ? sl * slab_it : it_small0 + (sl - n_big); };
+        auto park = [&](double *rec, const Acc<D> &sa, const Lse3 &sx) {
+            if (lane_rec) { rec[lane] = sa.w.m; rec[32 + lane] = sa.w.s; rec[64 + lane] = sa.w.q; }
+            else warp_reduce_to_slab<D, APF>(sa, sx, mom, rec, lane);
+        };
         // software pipeline (1-D states): the inputs of the next iteration -- of this slab, or of the slab the warp
         // takes next -- are requested before the current iteration's arithmetic starts (77.5 vs 80.8 us at 512
         // threads; at 768 threads / 80 registers it spills: 120 us)
         constexpr bool PREF = (D == 1);
-        int sl = grab();
-        In pre;
-        bool have = false;
-        if (PREF && sl < n_slab && fast_ok && first_it(sl) < n_full) { load_full(first_it(sl), pre); have = true; }
-        while (sl < n_slab) {
-            const int i0 = first_it(sl);
-            const int rem = it_small0 - i0;
-            const int cnt = sl < n_big ? (rem < slab_it ? rem : slab_it) : 1;
-            Acc<D> sa;
-            acc_init(sa);
-            Lse3 sx = lse3_empty();
-            int nsl = n_slab;
-            for (int k_ = 0; k_ < cnt; k_++) {
-                const int i = i0 + k_;
-                In cur;
-                const bool cur_have = have;
-                if (PREF && have) cur = pre;
-                int inext = -1;
-                if (k_ + 1 < cnt) inext = i + 1;
-                else { nsl = grab(); if (nsl < n_slab) inext = first_it(nsl); }
-                have = false;
-                if (PREF && inext >= 0 && fast_ok && inext < n_full) { load_full(inext, pre); have = true; }
-                if (PREF && cur_have) compute_full(i, cur, sa, sx);
-                else iteration(i, sa, sx);
+        // FUSED: every iteration runs step t and then step t + 1 on the values step t has just stored -- exactly what
+        // the unfused step t + 1 would load -- with the same slabs, lanes and batches, so both steps' records and
+        // partial rows carry the bits of two separate launches.  Step t + 1's records go to the CTA's slice of
+        // fuse_slab (the shared-memory buffer holds step t's).  In place: step t + 1 writes buffers [(t+1) & 1] =
+        // [(t-1) & 1], the pass's input.  Every element is read once, by the thread that later overwrites it, and its
+        // store depends on that load, so no thread ever reads a value another thread wrote; these loads therefore go
+        // through plain pointers (no __restrict__, no non-coherent loads).
+        auto slabs = [&](auto fused) {
+            constexpr bool FUSED = decltype(fused)::value;
+            // (no prefetch in a fused pair: its two steps of arithmetic per load cover the load latency, and the
+            // registers of a prefetched iteration would spill)
+            constexpr bool PF = PREF && !FUSED;
+            const StepIo io1 = FUSED ? step_io(a, t + 1, NZ) : io0;
+            const double *Xs = FUSED ? a.X[cur] : Xi;
+            const double *lws = FUSED ? a.lw[cur] : lwi;
+            const double *Xs_c = FUSED ? Xs + 2 * pstart : Xi_c;
+            const double *lws_c = FUSED ? lws + 2 * pstart : lwi_c;
+            double *const slab1 = FUSED ? a.fuse_slab + (size_t)blockIdx.x * StepCfg<M>::kSlabDoubles : nullptr;
+            int sl = grab();
+            In pre;
+            bool have = false;
+            if (PF && sl < n_slab && fast_ok && first_it(sl) < n_full) {
+                load_full(Xs_c, lws_c, first_it(sl), pre);
+                have = true;
             }
-            double *rec = s_slab + (size_t)sl * a.slab_stride;
-            if (lane_rec) { rec[lane] = sa.w.m; rec[32 + lane] = sa.w.s; rec[64 + lane] = sa.w.q; }
-            else warp_reduce_to_slab<D, APF>(sa, sx, mom, rec, lane);
-            sl = nsl;
+            while (sl < n_slab) {
+                const int i0 = first_it(sl);
+                const int rem = it_small0 - i0;
+                const int cnt = sl < n_big ? (rem < slab_it ? rem : slab_it) : 1;
+                Acc<D> sa, sb;
+                acc_init(sa);
+                Lse3 sx = lse3_empty(), sy = lse3_empty();
+                if (FUSED) acc_init(sb);
+                int nsl = n_slab;
+                for (int k_ = 0; k_ < cnt; k_++) {
+                    const int i = i0 + k_;
+                    In cin;
+                    const bool cur_have = have;
+                    if (PF && have) cin = pre;
+                    int inext = -1;
+                    if (k_ + 1 < cnt) inext = i + 1;
+                    else { nsl = grab(); if (nsl < n_slab) inext = first_it(nsl); }
+                    have = false;
+                    if (PF && inext >= 0 && fast_ok && inext < n_full) { load_full(Xs_c, lws_c, inext, pre); have = true; }
+                    const bool full = fast_ok && i < n_full;
+                    if (!(PF && cur_have)) {
+                        if (full) load_full(Xs_c, lws_c, i, cin);
+                        else load_general(Xs, lws, i, cin);
+                    }
+                    double l[2 * kU], x[2 * kU][D];
+                    if (full) compute_full(io0, i, cin, sa, sx, l, x);
+                    else compute_general(io0, i, cin, sa, sx, l, x);
+                    if (FUSED) {
+                        In nx;
+#pragma unroll
+                        for (int u = 0; u < kU; u++) {
+#pragma unroll
+                            for (int j2 = 0; j2 < 2; j2++) {
+                                nx.base[u][j2] = l[2 * u + j2];
+#pragma unroll
+                                for (int c = 0; c < D; c++) nx.xp[u][j2][c] = x[2 * u + j2][c];
+                            }
+                            // the odd last particle: load_general's (unused) base of the missing partner
+                            if (!full && 2 * (pstart + (int64_t)i * kIt + u * 32 + lane) + 1 == n) nx.base[u][1] = 0.0;
+                        }
+                        if (full) compute_full(io1, i, nx, sb, sy, l, x);
+                        else compute_general(io1, i, nx, sb, sy, l, x);
+                    }
+                }
+                park(s_stage + (size_t)sl * a.slab_stride, sa, sx);
+                if (FUSED) park(slab1 + (size_t)sl * a.slab_stride, sb, sy);
+                sl = nsl;
+            }
+        };
+        if constexpr (D == 1) {
+            if (fuse) slabs(std::true_type{});
+            else slabs(std::false_type{});
+        } else {
+            slabs(std::false_type{});
         }
         if (!speculate) goto step_done;
         // now the peers' statistics: bookkeeping, and was the guess right?
@@ -1468,7 +1574,7 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
                 if (!odd) acc_add_batch<2, D, true>(acc, l, x, mom);
                 else acc_add_batch<2, D, false>(acc, l, x, mom);
             } else {
-                do_pair(p, xp, base, x, l, av);
+                do_pair(io0, p, xp, base, x, l, av);
                 acc_add_batch<2, D>(acc, l, x, mom);
             }
             if (APF) lse3_add_batch<2>(aux, av);
@@ -1834,6 +1940,9 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
     }
 step_done:
     write_partial<D, APF, BS>(a, t, acc, aux, mom, sh, s_stage, n_slab);
+    if (fuse)   // (acc, aux: still empty -- the streaming branch keeps its statistics in the slab records)
+        write_partial<D, APF, BS>(a, t + 1, acc, aux, mom, sh, a.fuse_slab + (size_t)blockIdx.x * StepCfg<M>::kSlabDoubles,
+                                  n_slab);
 }
 
 // the prologue alone (one CTA): finalises the last enqueued step so that the host can read its summaries
