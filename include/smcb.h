@@ -327,6 +327,51 @@ typedef struct {
 /* ONE kernel launch for the whole backward pass (plus a memset of counts for reject); no host sync */
 int smcb_backward_sample(smcb_ctx *ctx, const smcb_smooth_desc *desc);
 
+/* ---------------------------------------------------------------------------
+ * on-line smoothing of additive functionals (particles/collectors.py:345-449): one step t >= 1 of the PaRIS and
+ * O(N^2) collectors.  The caller evaluates the user's add_func psi between the launches.
+ * ------------------------------------------------------------------------- */
+#define SMCB_ONLINE_PARIS 0     /* B[n, i] ~ p(a | x_t^n) prop. to W_{t-1}[a] p_t(x_t^n | x_{t-1}^a), j = n*Np + i:
+                                   at most max_trials proposals a ~ W_{t-1} accepted w.p. p_t / C_t, then the
+                                   exact O(N) draw (hybrid PaRIS, Dau & Chopin 2022) */
+#define SMCB_ONLINE_ON2_W 1     /* omega (rows, N): omega[r, m] = W_{t-1}[m] p_t(x_t^{row0+r} | x_{t-1}^m), normalised
+                                   per row */
+#define SMCB_ONLINE_PHI_PARIS 2 /* phi[n] = (sum_i phi_prev[B[n, i]] + psi[n, i]) / Np  (model ignored) */
+#define SMCB_ONLINE_PHI_ON2 3   /* phi[r] = sum_m omega[r, m] (phi_prev[m] + psi[r, m]) / sum_m omega[r, m] */
+
+typedef struct {
+    int32_t method, model, dim, n_params;
+    int64_t t;                 /* the time of X; the density is logpt(t, X_prev, X) */
+    int64_t N;                 /* particles at t - 1 and t                                          */
+    int64_t Np;                /* PaRIS: draws per particle (Nparis)                                 */
+    int64_t max_trials;        /* PaRIS: proposals per draw before the exact draw                     */
+    int64_t row0, rows;        /* ON2: the block of rows [row0, row0 + rows) of X                     */
+    int64_t k;                 /* PHI: components of phi / psi                                        */
+    uint64_t seed;             /* PaRIS: Philox key; the draws are keyed by (seed, t, j, trial)         */
+    double log_bound;          /* PaRIS: log C_t >= log p_t(x | xp)                                   */
+    double step_const;         /* the model's per-step constant of step t (Gordon_etal), else 0        */
+    double params[SMCB_MAX_PARAMS];  /* model constants, same layout as smcb_filter_desc.params         */
+    /* X_{t-1} and X_t: particle n, component c at X[n * x_stride_n + c * x_stride_c] (element strides) */
+    const double *X_prev;
+    const double *X;
+    int64_t x_stride_n, x_stride_c;
+    const double *lw_prev;     /* (N) log-weights of t - 1                                            */
+    const double *cdf;         /* PaRIS: (N) inclusive prefix sum of W_{t-1} (any positive scale)      */
+    /* injected randomness (parity tests) or NULL: prop / lu (N, Np, max_trials), u_exact (N, Np)     */
+    const int64_t *prop;
+    const double *lu;
+    const double *u_exact;
+    int64_t *B;                /* PaRIS: out (N, Np); PHI_PARIS: in                                    */
+    int64_t *counts;           /* PaRIS: {accepted, proposals} += this step's (integer atomics)        */
+    double *omega;             /* ON2_W: out (rows, N); PHI_ON2: in                                    */
+    const double *phi_prev;    /* PHI: (N, k)                                                          */
+    const double *psi;         /* PHI_PARIS: (N, Np, k); PHI_ON2: (rows, N, k)                         */
+    double *phi;               /* PHI: out (rows, k) (PARIS: rows = N)                                 */
+} smcb_online_desc;
+
+/* one kernel launch, no host sync */
+int smcb_online_smooth(smcb_ctx *ctx, const smcb_online_desc *desc);
+
 #ifdef __cplusplus
 }
 #endif

@@ -53,6 +53,21 @@ class SmoothDesc(C.Structure):
     ]
 
 
+ONLINE_PARIS, ONLINE_ON2_W, ONLINE_PHI_PARIS, ONLINE_PHI_ON2 = 0, 1, 2, 3
+
+
+class OnlineDesc(C.Structure):
+    _fields_ = [
+        ("method", C.c_int32), ("model", C.c_int32), ("dim", C.c_int32), ("n_params", C.c_int32),
+        ("t", C.c_int64), ("N", C.c_int64), ("Np", C.c_int64), ("max_trials", C.c_int64),
+        ("row0", C.c_int64), ("rows", C.c_int64), ("k", C.c_int64), ("seed", C.c_uint64),
+        ("log_bound", C.c_double), ("step_const", C.c_double), ("params", C.c_double * SMCB_MAX_PARAMS),
+        ("X_prev", c_dp), ("X", c_dp), ("x_stride_n", C.c_int64), ("x_stride_c", C.c_int64),
+        ("lw_prev", c_dp), ("cdf", c_dp), ("prop", c_dp), ("lu", c_dp), ("u_exact", c_dp),
+        ("B", c_dp), ("counts", c_dp), ("omega", c_dp), ("phi_prev", c_dp), ("psi", c_dp), ("phi", c_dp),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/smcb.h declares
 PROTOTYPES = {
     "smcb_last_error": (C.c_char_p, []),
@@ -110,6 +125,7 @@ PROTOTYPES = {
     "smcb_filter_state": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),
     "smcb_filter_fusion_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "smcb_backward_sample": (C.c_int, [C.c_void_p, C.POINTER(SmoothDesc)]),
+    "smcb_online_smooth": (C.c_int, [C.c_void_p, C.POINTER(OnlineDesc)]),
 }
 
 _lib = None

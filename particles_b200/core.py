@@ -323,7 +323,8 @@ class SMC:
         spec = None
         if fused is not False:
             from .state_space_models import fused_spec
-            spec = fused_spec(fk)
+            # a model that only adds the smoothing hooks to a stock class runs fused when it is smoothed on-line
+            spec = fused_spec(fk, smoothing_hooks=self.summaries is not None and bool(self.summaries.online))
             if spec is not None and resampling not in _lib.FUSED_SCHEMES:
                 spec = None                      # residual, ssp, killing, ...: plugin path (stand-alone kernels)
             if spec is None and fused is True:
@@ -352,6 +353,17 @@ class SMC:
         if t not in self._row_cache:
             self._row_cache = {t: self._engine.summ[t].cpu().numpy()}
         return self._row_cache[t]
+
+    def _engine_gen(self, t):
+        """Generation t of the fused filter as the on-line smoothers read it, after step t and before step t + 2
+        (step s writes buffers [s & 1]): views of the device buffers, and the ancestors chosen on the device from
+        the step's resampling flag -- no host sync."""
+        e = self._engine
+        x = e.X[t & 1]
+        A = None
+        if t > 0:
+            A = torch.where(e.summ[t, 2] != 0, e.A, torch.arange(self.N, device=e.A.device))
+        return collectors._Gen(t, x if x.ndim == 1 else x.t(), e.lw[t & 1], A)
 
     def _cur(self):
         return (self._done - 1) & 1      # step s writes buffers [s & 1]
@@ -546,12 +558,23 @@ class SMC:
         """Run until completion (core.py:391-409); ``cpu_time`` is the wall time of this
         call, device work included (utils.timer semantics, utils.py:81-89)."""
         t0 = time.perf_counter()
+        online = [] if self.summaries is None else self.summaries.online
         if self.fused and not self.verbose and not self.hist \
-                and (self.summaries is None or self.summaries.only_defaults or self._dev_moments) \
+                and (self.summaries is None or self.summaries.only_defaults or self._dev_moments
+                     or len(online) == len(self.summaries._collectors) - self.summaries._n_default) \
                 and getattr(getattr(type(self.fk), "done", None), "__qualname__", "") == "FeynmanKac.done":
             T = self._engine.T
             first = self.t
-            if first < T:
+            if online:
+                # one-step batches: generation t - 1 stays intact in buffers (t - 1) & 1 while the smoothers read
+                # it after step t (a batch of one step never fuses two steps)
+                for t in range(first, T):
+                    self._engine.step(1)
+                    self.t, self._done = t, t + 1
+                    for col in online:
+                        col._advance(self.fk, self._seed, self._engine_gen(t))
+                self.t = self._done = T
+            elif first < T:
                 self._engine.step(T - first)
                 self.t = self._done = T
             table = self._engine.summ.cpu().numpy()       # the one device->host read of the run
@@ -562,6 +585,8 @@ class SMC:
                                                 [bool(v) for v in table[first:T, 2]])
                 if self._dev_moments:
                     self.summaries._extend_moments(self._engine.mom.cpu().numpy()[first:T], self._engine.dim)
+                for col in online:
+                    col._flush()
         else:
             for _ in self:
                 pass

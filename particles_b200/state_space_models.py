@@ -57,6 +57,10 @@ class StateSpaceModel:
         """state_space_models.py:261-266: log of a constant C_t >= p(x_t | x_{t-1}) (rejection smoothing)."""
         raise NotImplementedError(err_msg_missing_cst % self.__class__.__name__)
 
+    def add_func(self, t, xp, x):
+        """state_space_models.py:268-270: the additive function psi_t(x_{t-1}, x_t) of on-line smoothing."""
+        raise NotImplementedError(self._error_msg("add_func"))
+
     def simulate_given_x(self, x):
         lag_x = [None] + x[:-1]
         return [self.PY(t, xp, xx).rvs(size=1) for t, (xp, xx) in enumerate(zip(lag_x, x))]
@@ -96,6 +100,10 @@ class Bootstrap(FeynmanKac):
     def upper_bound_trans(self, t):
         """state_space_models.py:345-346."""
         return self.ssm.upper_bound_log_pt(t)
+
+    def add_func(self, t, xp, x):
+        """state_space_models.py:348-349."""
+        return self.ssm.add_func(t, xp, x)
 
 
 class GuidedPF(Bootstrap):
@@ -397,19 +405,37 @@ _SPECS = {"StochVol": spec_stochvol, "LinearGauss": spec_lingauss, "Gordon_etal"
           "StochVolLeverage": spec_stochvollev, "DiscreteCox": spec_discretecox}
 
 
-def fused_spec(fk):
+_SMOOTHING_HOOKS = {"add_func", "upper_bound_log_pt", "upper_bound_trans"}
+_INERT = {"__module__", "__qualname__", "__doc__", "__dict__", "__weakref__", "__firstlineno__",
+          "__static_attributes__"}
+
+
+def _hooks_base(cls):
+    """``cls``, or -- when it adds nothing to its single base but the smoothing hooks, which the filter never
+    calls -- that base, recursively."""
+    while len(cls.__bases__) == 1 and not (set(cls.__dict__) - _SMOOTHING_HOOKS - _INERT):
+        cls = cls.__bases__[0]
+    return cls
+
+
+def fused_spec(fk, smoothing_hooks=False):
     """Return the fused-kernel description of ``fk`` or None if it is not a stock
     (Feynman-Kac kind, model) pair.  Only exact stock classes are recognised: a user
     subclass that overrides a closure has another class name or module and takes the
-    generic plugin path instead."""
-    names = [c.__name__ for c in type(fk).__mro__]
+    generic plugin path instead.  With ``smoothing_hooks`` (the run smooths on-line), a
+    subclass that adds only ``add_func``, ``upper_bound_log_pt`` or ``upper_bound_trans``
+    to a stock class counts as that class."""
+    base = _hooks_base if smoothing_hooks else (lambda c: c)
+    fk_cls = base(type(fk))
+    names = [c.__name__ for c in fk_cls.__mro__]
     kind = next((code for nm, code in _FK_KINDS if nm in names), None)
-    if kind is None or type(fk).__name__ not in [k for k, _ in _FK_KINDS]:
+    if kind is None or fk_cls.__name__ not in [k for k, _ in _FK_KINDS]:
         return None
     ssm = getattr(fk, "ssm", None)
-    if ssm is None or type(ssm).__module__ not in _TRUSTED_MODULES:
+    ssm_cls = None if ssm is None else base(type(ssm))
+    if ssm is None or ssm_cls.__module__ not in _TRUSTED_MODULES:
         return None
-    make = _SPECS.get(type(ssm).__name__)
+    make = _SPECS.get(ssm_cls.__name__)
     if make is None:
         return None
     spec = make(ssm, fk.T, fk.data) if make in (spec_mvlingauss, spec_discretecox) else make(ssm, fk.T)
