@@ -372,6 +372,39 @@ typedef struct {
 /* one kernel launch, no host sync */
 int smcb_online_smooth(smcb_ctx *ctx, const smcb_online_desc *desc);
 
+/* ---------------------------------------------------------------------------
+ * genealogy-based variance estimators (particles/variance_estimators.py:93-201): the Eve indices of a running filter
+ * and the branch sums  sum_b (sum_{m: B_m = b} v_m)^2  over SORTED rows B, so that each branch is a contiguous run.
+ * ------------------------------------------------------------------------- */
+#define SMCB_VAR_EVE 0          /* if the step resampled: B[p ^ 1][n] = B[p][A[n]], p = *parity (one launch) */
+#define SMCB_VAR_SUMS 1         /* the branch sums of L rows, k components each (four launches, then *parity ^= rs) */
+#define SMCB_VAR_CENTRED 0      /* v = W (phi - m), m = sum W phi / sum W; zeros where B[0] == B[N-1] (Var)    */
+#define SMCB_VAR_WEIGHTS 1      /* v = W, no centring and no zero rule (Var_logLt)                              */
+
+typedef struct {
+    int32_t method, mode;
+    int32_t lin_w;             /* lw holds the weights W themselves (var_estimate), else log-weights: W = exp(lw) / sum */
+    int32_t rs_host;           /* the step's resampling flag when rs_flag is NULL                                */
+    int64_t N, k, L;           /* particles, components of phi (1 in WEIGHTS mode), rows of B                     */
+    const double *rs_flag;     /* device: the step resampled when nonzero (the filter's summaries[t, 2]), or NULL */
+    int32_t *parity;           /* device word: the Eve row is B[*parity] (B[*parity ^ rs] after EVE); NULL: B[0]   */
+    int64_t *B[2];             /* EVE: the ping-pong pair of (N) rows; SUMS: (L, N) rows at B[cur]              */
+    const int64_t *A;          /* EVE: the step's ancestors (read only when the step resampled)                  */
+    const double *lw;          /* SUMS: (N) log-weights (or W), the mean and the normaliser                       */
+    const double *phi;         /* SUMS, CENTRED: (N, k) row-major                                                */
+    const double *lw_rows;     /* SUMS: row r reads lw_rows + r * row_ld and phi_rows + r * row_ld * k           */
+    const double *phi_rows;
+    int64_t row_ld;            /* 0 when every row reads lw and phi (sorted rows)                                 */
+    const uint8_t *zero;       /* CENTRED: (L) the B[0] == B[N-1] rule decided by the caller, or NULL: on the row */
+    int32_t *unsorted;         /* (L) set to 1 when a row is not sorted (never cleared here)                      */
+    double *scratch;           /* smcb_variance_scratch_doubles(N, L, k) doubles                                   */
+    double *out;               /* (L, k) the estimates                                                            */
+} smcb_variance_desc;
+
+/* no host sync; the chunk size is a function of N only, so the bits do not depend on the device */
+int smcb_variance(smcb_ctx *ctx, const smcb_variance_desc *desc);
+int64_t smcb_variance_scratch_doubles(int64_t N, int64_t L, int64_t k);
+
 #ifdef __cplusplus
 }
 #endif

@@ -68,6 +68,20 @@ class OnlineDesc(C.Structure):
     ]
 
 
+VAR_EVE, VAR_SUMS = 0, 1
+VAR_CENTRED, VAR_WEIGHTS = 0, 1
+
+
+class VarDesc(C.Structure):
+    _fields_ = [
+        ("method", C.c_int32), ("mode", C.c_int32), ("lin_w", C.c_int32), ("rs_host", C.c_int32),
+        ("N", C.c_int64), ("k", C.c_int64), ("L", C.c_int64),
+        ("rs_flag", c_dp), ("parity", c_dp), ("B", c_dp * 2), ("A", c_dp), ("lw", c_dp), ("phi", c_dp),
+        ("lw_rows", c_dp), ("phi_rows", c_dp), ("row_ld", C.c_int64), ("zero", c_dp), ("unsorted", c_dp),
+        ("scratch", c_dp), ("out", c_dp),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/smcb.h declares
 PROTOTYPES = {
     "smcb_last_error": (C.c_char_p, []),
@@ -126,6 +140,8 @@ PROTOTYPES = {
     "smcb_filter_fusion_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "smcb_backward_sample": (C.c_int, [C.c_void_p, C.POINTER(SmoothDesc)]),
     "smcb_online_smooth": (C.c_int, [C.c_void_p, C.POINTER(OnlineDesc)]),
+    "smcb_variance": (C.c_int, [C.c_void_p, C.POINTER(VarDesc)]),
+    "smcb_variance_scratch_doubles": (C.c_int64, [C.c_int64, C.c_int64, C.c_int64]),
 }
 
 _lib = None

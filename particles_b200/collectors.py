@@ -6,7 +6,9 @@ device table the kernels write, so they cost no per-step host sync.
 
 The on-line smoothers of additive functionals (``Online_smooth_naive``, ``Online_smooth_ON2``, ``Paris``) keep
 Phi on the device; their per-step work is csrc/smcb_online.cu plus the user's ``add_func``, and their summaries
-are read from the device in one transfer per ``collect`` (per step) or per fused ``run()``.
+are read from the device in one transfer per ``collect`` (per step) or per fused ``run()``.  The variance
+collectors ``Var`` and ``Var_logLt`` (variance_estimators.py) share that row buffer.  ``Fixed_lag_smooth`` reads
+the rolling history (``store_history=k``).
 """
 import ctypes as C
 
@@ -98,16 +100,34 @@ def _gen_of(smc):
     return _Gen(smc.t, as_device(smc.X), as_device(smc.wgts.lw), smc.A)
 
 
-class OnlineSmootherMixin:
+class DeviceRowsMixin:
+    """Collectors whose per-step work stays on the device: ``_step(smc, t)`` enqueues the work of step t and appends
+    one device row to ``_rows`` (no host sync); ``_flush`` moves the rows into ``summary`` in one transfer -- per step
+    in ``collect``, once per run in the fused ``SMC.run()``.  A row is a float summary, or a (k,) array when
+    ``_vector``."""
+
+    def collect(self, smc):
+        self._step(smc, smc.t)
+        self._flush()
+
+    def _flush(self):
+        """Move the rows enqueued since the last flush into ``summary`` (one device-to-host transfer)."""
+        if not self._rows:
+            return
+        rows = torch.stack(self._rows).cpu().numpy()
+        self._rows = []
+        self.summary.extend(r.copy() if self._vector else float(r[0]) for r in rows)
+
+
+class OnlineSmootherMixin(DeviceRowsMixin):
     """collectors.py:345-365: Phi_0 = add_func(0, None, X_0), then the class's ``update``; each step appends the
     weighted mean of Phi under W_t -- a float when Phi is (N,), a (k,) array when Phi is (N, k).
 
     Calling convention of ``add_func`` here: CUDA fp64 tensors ``xp`` and ``x`` of the same shape, (K,) or (K, d),
     returning (K,) or (K, k) (``xp`` is None at t = 0).  ON2 and PaRIS call it on flattened pairs."""
 
-    def collect(self, smc):
-        self._advance(smc.fk, smc._seed, _gen_of(smc))
-        self._flush()
+    def _step(self, smc, t):
+        self._advance(smc.fk, smc._seed, smc._engine_gen(t) if smc.fused else _gen_of(smc))
 
     def _advance(self, fk, seed, g):
         """Enqueue the work of step g.t (no host sync)."""
@@ -121,14 +141,6 @@ class OnlineSmootherMixin:
         W = rs.exp_and_normalise(g.lw)
         self._rows.append((W[:, None] * self._Phi).sum(0) / W.sum())   # np.average(Phi, axis=0, weights=W)
         self._prev, self._prev_W = g, W
-
-    def _flush(self):
-        """Move the rows enqueued since the last flush into ``summary`` (one device-to-host transfer)."""
-        if not self._rows:
-            return
-        rows = torch.stack(self._rows).cpu().numpy()
-        self._rows = []
-        self.summary.extend(r.copy() if self._vector else float(r[0]) for r in rows)
 
     def update(self, fk, seed, g):
         raise NotImplementedError
@@ -254,7 +266,7 @@ class Paris(OnlineSmootherMixin, Collector):
         self._counts = []
 
     def _flush(self):
-        OnlineSmootherMixin._flush(self)
+        DeviceRowsMixin._flush(self)
         if self._counts:
             c = torch.stack(self._counts).cpu().numpy()
             self._counts = []
@@ -330,15 +342,53 @@ class Paris(OnlineSmootherMixin, Collector):
         counts[1] = nprops
 
 
+def _lw_of(smc):
+    """The log-weights of the current generation, on the device."""
+    if smc.fused:
+        return smc._engine.lw[smc._cur()]
+    return as_device(smc.wgts.lw).contiguous()
+
+
+class Fixed_lag_smooth(Collector):
+    """collectors.py:324-342: with ``store_history=k``, the weighted mean under W_t of ``phi`` of the fixed-lag
+    trajectories.  ``phi`` receives the list of the ``hist.T`` CUDA tensors X_s[B[s]] (B =
+    ``hist.compute_trajectories()``) and returns (N,); the summary is a float.  Without ``phi`` it raises TypeError,
+    as the reference's ``np.average`` of a list of arrays does."""
+    signature = {"phi": None}
+
+    def fetch(self, smc):
+        if self.phi is None:
+            raise TypeError("Fixed_lag_smooth: phi must map the list of fixed-lag particle arrays to an (N,) array")
+        B = smc.hist.compute_trajectories()
+        Xs = [as_device(X)[B[i]] for i, X in enumerate(smc.hist.X)]
+        lw = _lw_of(smc)
+        v = as_device(self.phi(Xs))
+        if v.shape != lw.shape:
+            raise ValueError(f"Fixed_lag_smooth: phi must return an array of shape {tuple(lw.shape)}, got "
+                             f"{tuple(v.shape)}")
+        W = rs.exp_and_normalise(lw)
+        return float(((W * v).sum() / W.sum()).item())           # np.average(phi(Xs), weights=W)
+
+
 _ONLINE = (Online_smooth_naive, Online_smooth_ON2, Paris)
-_REF_ONLINE = {c.__name__: c for c in _ONLINE}
+_REF_COLLECTORS = {c.__name__: c for c in _ONLINE + (Fixed_lag_smooth,)}
+
+
+def _ref_classes(module):
+    if module == "particles.collectors":
+        return _REF_COLLECTORS
+    if module == "particles.variance_estimators":
+        from . import variance_estimators as ve
+        return {c.__name__: c for c in (ve.Var, ve.Var_logLt, ve.Lag_based_var)}
+    return {}
 
 
 def _native(col):
-    """The reference's own on-line smoothing collectors (particles.collectors) -> ours, same keyword arguments."""
+    """The reference's own on-line smoothing, fixed-lag and variance collectors (particles.collectors,
+    particles.variance_estimators) -> ours, same keyword arguments."""
     cls = type(col)
-    if cls.__module__ == "particles.collectors" and cls.__name__ in _REF_ONLINE:
-        ours = _REF_ONLINE[cls.__name__]
+    ours = _ref_classes(cls.__module__).get(cls.__name__)
+    if ours is not None:
         return ours(**{k: getattr(col, k) for k in getattr(cls, "signature", {}) if k in ours.signature})
     return col()
 
@@ -363,11 +413,16 @@ class Summaries:
         """The on-line smoothers among the collectors."""
         return [c for c in self._collectors[self._n_default:] if isinstance(c, OnlineSmootherMixin)]
 
+    @property
+    def device_rows(self):
+        """The collectors whose per-step work stays on the device (on-line smoothers, ``Var``, ``Var_logLt``)."""
+        return [c for c in self._collectors[self._n_default:] if isinstance(c, DeviceRowsMixin)]
+
     def device_moments(self, fk):
-        """True when every non-default collector other than the on-line smoothers is ``Moments()`` with the default
-        ``mom_func`` and the model keeps ``FeynmanKac.default_moments`` (resampling.wmean_and_var): exactly what the
-        fused step kernel accumulates."""
-        extra = [c for c in self._collectors[self._n_default:] if not isinstance(c, OnlineSmootherMixin)]
+        """True when every non-default collector other than the device-row collectors (on-line smoothers, ``Var``,
+        ``Var_logLt``) is ``Moments()`` with the default ``mom_func`` and the model keeps
+        ``FeynmanKac.default_moments`` (resampling.wmean_and_var): exactly what the fused step kernel accumulates."""
+        extra = [c for c in self._collectors[self._n_default:] if not isinstance(c, DeviceRowsMixin)]
         if not extra or not all(type(c) is Moments and c.mom_func is None for c in extra):
             return False
         dm = getattr(type(fk), "default_moments", None)

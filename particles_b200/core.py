@@ -558,7 +558,7 @@ class SMC:
         """Run until completion (core.py:391-409); ``cpu_time`` is the wall time of this
         call, device work included (utils.timer semantics, utils.py:81-89)."""
         t0 = time.perf_counter()
-        online = [] if self.summaries is None else self.summaries.online
+        online = [] if self.summaries is None else self.summaries.device_rows
         if self.fused and not self.verbose and not self.hist \
                 and (self.summaries is None or self.summaries.only_defaults or self._dev_moments
                      or len(online) == len(self.summaries._collectors) - self.summaries._n_default) \
@@ -572,7 +572,7 @@ class SMC:
                     self._engine.step(1)
                     self.t, self._done = t, t + 1
                     for col in online:
-                        col._advance(self.fk, self._seed, self._engine_gen(t))
+                        col._step(self, t)
                 self.t = self._done = T
             elif first < T:
                 self._engine.step(T - first)
