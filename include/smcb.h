@@ -405,6 +405,43 @@ typedef struct {
 int smcb_variance(smcb_ctx *ctx, const smcb_variance_desc *desc);
 int64_t smcb_variance_scratch_doubles(int64_t N, int64_t L, int64_t k);
 
+/* ---------------------------------------------------------------------------
+ * batched filters (multiSMC): R independent filters of the same model, Feynman-Kac kind, scheme, N and T in ONE
+ * launch, one CTA per filter (csrc/smcb_batch.cu).  1-D fused models only.  Run r draws what the single filter
+ * with seed seed[r] draws (same Philox counters); the two differ only in reduction order.
+ * Per-run rows are padded to ld = N rounded up to even (16-byte aligned rows).
+ * ------------------------------------------------------------------------- */
+#define SMCB_BATCH_AUTO 0      /* resident if the filter fits in shared memory, else streaming */
+#define SMCB_BATCH_RESIDENT 1  /* x, lw and the CDF stay in shared memory for the whole run     */
+#define SMCB_BATCH_STREAMING 2 /* per-run buffers in device memory; any N                       */
+
+typedef struct {
+    int32_t model, fk, scheme, dim;  /* dim must be 1                                              */
+    int32_t dy, n_params;
+    int32_t tier, reserved0;         /* SMCB_BATCH_*                                               */
+    int64_t N, T, R;
+    const uint64_t *seed;      /* (R) Philox key of each run                                        */
+    const double *essrmin;     /* (R)                                                               */
+    const double *params;      /* (R, n_params) model constants, layout of smcb_filter_desc.params  */
+    const double *data;        /* (R, T, dy) observations                                           */
+    const double *step_consts; /* (R, T) or NULL                                                    */
+    double *X;                 /* (R, 2, ld): generation s of the last two in X[r][s & 1]           */
+    double *lw;                /* (R, ld) log-weights of step T - 1                                 */
+    int64_t *A;                /* (R, ld) ancestors of step T - 1 (written only if it resampled)    */
+    double *cdf;               /* streaming: (R, ld) scratch; resident: unused                      */
+    double *scratch;           /* streaming multinomial: (R, ld + 2) exponential spacings           */
+    double *summaries;         /* (R, T, SMCB_SUMMARY_STRIDE)                                       */
+    double *moments;           /* NULL, or (R, T, 8) as smcb_filter_desc.moments                    */
+    const double *z_in;        /* NULL, or injected N(0,1): (R, T, n_noise, N)                      */
+    const double *u_in;        /* NULL, or injected uniforms: (R, T, N + 1)                         */
+} smcb_batch_desc;
+
+/* out[0] = the tier a run with this descriptor takes, out[1] = its grid (CTAs).  Reads only the shape fields.
+ * SMCB_ENOSYS for a combination that is not built (the caller runs those filters one by one). */
+int smcb_batch_plan(smcb_ctx *ctx, const smcb_batch_desc *desc, int64_t out[2]);
+/* one launch on the context's stream, no host sync */
+int smcb_batch_run(smcb_ctx *ctx, const smcb_batch_desc *desc);
+
 #ifdef __cplusplus
 }
 #endif

@@ -4,7 +4,7 @@ Hand-written sm_90a CUDA kernels (csrc/, C-ABI in include/smcb.h) behind the
 reference's own plugin surface: ``SMC``, ``FeynmanKac``, ``state_space_models``,
 ``distributions``, ``resampling``, ``collectors``.  See DESIGN.md / INTEGRATION.md.
 """
-from .core import SMC, FeynmanKac  # noqa: F401
+from .core import SMC, FeynmanKac, multiSMC  # noqa: F401
 from .device import seed  # noqa: F401
 
 __version__ = "0.1.0"

@@ -82,6 +82,20 @@ class VarDesc(C.Structure):
     ]
 
 
+BATCH_AUTO, BATCH_RESIDENT, BATCH_STREAMING = 0, 1, 2
+
+
+class BatchDesc(C.Structure):
+    _fields_ = [
+        ("model", C.c_int32), ("fk", C.c_int32), ("scheme", C.c_int32), ("dim", C.c_int32),
+        ("dy", C.c_int32), ("n_params", C.c_int32), ("tier", C.c_int32), ("reserved0", C.c_int32),
+        ("N", C.c_int64), ("T", C.c_int64), ("R", C.c_int64),
+        ("seed", c_dp), ("essrmin", c_dp), ("params", c_dp), ("data", c_dp), ("step_consts", c_dp),
+        ("X", c_dp), ("lw", c_dp), ("A", c_dp), ("cdf", c_dp), ("scratch", c_dp),
+        ("summaries", c_dp), ("moments", c_dp), ("z_in", c_dp), ("u_in", c_dp),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/smcb.h declares
 PROTOTYPES = {
     "smcb_last_error": (C.c_char_p, []),
@@ -142,6 +156,8 @@ PROTOTYPES = {
     "smcb_online_smooth": (C.c_int, [C.c_void_p, C.POINTER(OnlineDesc)]),
     "smcb_variance": (C.c_int, [C.c_void_p, C.POINTER(VarDesc)]),
     "smcb_variance_scratch_doubles": (C.c_int64, [C.c_int64, C.c_int64, C.c_int64]),
+    "smcb_batch_plan": (C.c_int, [C.c_void_p, C.POINTER(BatchDesc), C.POINTER(C.c_int64)]),
+    "smcb_batch_run": (C.c_int, [C.c_void_p, C.POINTER(BatchDesc)]),
 }
 
 _lib = None

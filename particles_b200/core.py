@@ -593,3 +593,320 @@ class SMC:
             if self.fused:
                 torch.cuda.synchronize()
         self.cpu_time = time.perf_counter() - t0
+
+
+# ---------------------------------------------------------------------------------------------------- multiSMC
+# Cost model of the routing rule, in seconds per filter step, measured with tools/bench_multismc.py on an NVIDIA H100
+# 80GB HBM3 at a 400 W power limit (DESIGN.md section 5.7):
+#   * one run of the single engine, end to end (construction, T steps, summary read) over T: LOOP_STEP, interpolated
+#     in log N between the measured points and clamped at both ends;
+#   * one wave of the batched kernel (every CTA runs one filter): BATCH_STEP_S + N * BATCH_PARTICLE_S in the resident
+#     tier; N * STREAM_PARTICLE_S in the streaming tier with one CTA per SM, times 1 + STREAM_SHARE for every further
+#     CTA that shares an SM (they split its memory bandwidth).
+LOOP_STEP = ((256, 11.9e-6), (4096, 12.6e-6), (16384, 13.0e-6), (65536, 15.1e-6), (131072, 19.0e-6),
+             (262144, 18.0e-6), (1048576, 119e-6), (10_000_000, 165e-6))
+BATCH_STEP_S, BATCH_PARTICLE_S = 3.6e-6, 1.6e-9
+STREAM_PARTICLE_S, STREAM_SHARE = 3.8e-9, 0.45
+
+
+def loop_step_s(N):
+    """Measured end-to-end cost of one single-engine step at N particles (LOOP_STEP, log-log interpolation)."""
+    xs = np.log([n for n, _ in LOOP_STEP])
+    ys = np.log([v for _, v in LOOP_STEP])
+    return float(np.exp(np.interp(np.log(max(N, 1)), xs, ys)))
+
+
+def batch_pays(N, R, tier, grid, n_sm=132):
+    """True when R filters of N particles finish sooner in batched launches -- ceil(R / grid) waves, one filter per
+    CTA -- than one after another through ``SMC``, by the measured cost model above."""
+    grid = max(int(grid), 1)
+    waves = -(-R // grid)
+    if tier == _lib.BATCH_RESIDENT:
+        wave = BATCH_STEP_S + N * BATCH_PARTICLE_S
+    else:
+        per_sm = -(-min(R, grid) // n_sm)
+        wave = N * STREAM_PARTICLE_S * (1 + STREAM_SHARE * (per_sm - 1))
+    return waves * wave < R * loop_step_s(N)
+
+
+_SMC_ARGS = {"fk", "N", "qmc", "resampling", "ESSrmin", "store_history", "verbose", "collect"}
+
+
+def batch_key(kw, _specs=None):
+    """(group key, fused spec) of a run that ``multiSMC`` can run in a batched launch, or (None, None) for a run
+    that takes the per-run path (``SMC(**kw, seed=seed).run()``).  ``kw`` are the run's ``SMC`` arguments.
+    The key holds what selects the kernel and the shapes; model constants, data and ``ESSrmin`` are per run."""
+    if set(kw) - _SMC_ARGS or kw.get("qmc") or kw.get("store_history") or kw.get("verbose"):
+        return None, None
+    fk, N = kw.get("fk"), int(kw.get("N", 100))
+    scheme = kw.get("resampling", "systematic")
+    if fk is None or scheme not in _lib.FUSED_SCHEMES or N < 1:
+        return None, None
+    if getattr(getattr(type(fk), "done", None), "__qualname__", "") != "FeynmanKac.done":
+        return None, None
+    from .state_space_models import fused_spec
+    if _specs is None:
+        spec = fused_spec(fk)
+    else:                                   # one spec per distinct Feynman-Kac object (its runs share it)
+        if id(fk) not in _specs:
+            _specs[id(fk)] = (fk, fused_spec(fk))
+        spec = _specs[id(fk)][1]
+    if spec is None or int(spec.get("dim", 1)) != 1 or int(spec.get("dy", 1)) != 1:
+        return None, None
+    collect = kw.get("collect")
+    moments = False
+    if collect != "off":
+        summ = collectors.Summaries(collect)
+        if not summ.only_defaults:
+            if summ.device_rows or not summ.device_moments(fk):
+                return None, None
+            moments = True
+    key = (spec["model"], spec["fk"], scheme, N, int(spec["data"].shape[0]), moments, collect == "off")
+    return key, spec
+
+
+class BatchRun:
+    """One filter of a batched ``multiSMC`` group, after its run: the attributes of ``SMC`` after ``run()``
+    (``t, N, fk, logLt, rs_flag, log_mean_w, loglt, X, Xp, A, wgts, W, summaries, cpu_time``) as views of the group's
+    device buffers of its chunk.  ``cpu_time`` is the wall time of the chunk (upload, launch, device work and the one
+    read of its summary table) divided by its number of runs: the cost per run of the batched launch.  ``summaries``
+    is built from the chunk's table on first access."""
+
+    def __init__(self, buf, i, fk, N, resampling, ESSrmin, seed, table, mom, collect, cpu_time):
+        self._buf, self._i = buf, i
+        self.fk, self.N, self.resampling, self.ESSrmin = fk, N, resampling, ESSrmin
+        self.qmc, self.verbose, self.hist, self.seed = False, False, None, seed
+        self.T = self.t = table.shape[0]
+        self._table, self._mom, self._collect = table, mom, collect
+        self._summaries = None
+        self.cpu_time = cpu_time
+
+    @property
+    def summaries(self):
+        if self._summaries is None and self._collect != "off":
+            sm = collectors.Summaries(self._collect)
+            t = self._table
+            sm._extend_defaults([float(v) for v in t[:, 0]], [float(v) for v in t[:, 1]], [bool(v) for v in t[:, 2]])
+            if self._mom is not None:
+                sm._extend_moments(self._mom, 1)
+            self._summaries = sm
+        return self._summaries
+
+    @property
+    def logLt(self):
+        return float(self._table[-1, 1])
+
+    @property
+    def rs_flag(self):
+        return bool(self._table[-1, 2])
+
+    @property
+    def log_mean_w(self):
+        return float(self._table[-1, 3])
+
+    @property
+    def loglt(self):
+        if self.T == 1 or self.rs_flag:
+            return self.log_mean_w
+        return self.log_mean_w - float(self._table[-2, 3])
+
+    def _gen(self, s):
+        return self._buf["X"][self._i, s & 1, :self.N]
+
+    @property
+    def X(self):
+        return self._gen(self.T - 1)
+
+    @property
+    def A(self):
+        if self.T <= 1:
+            return None
+        if self.rs_flag:
+            return self._buf["A"][self._i, :self.N]
+        return torch.arange(self.N, device=self._buf["A"].device)
+
+    @property
+    def Xp(self):
+        if self.T <= 1:
+            return None
+        prev = self._gen(self.T - 2)
+        if not self.rs_flag:
+            return prev
+        ctx = context()
+        out = torch.empty_like(prev)
+        _lib.check(ctx.lib.smcb_gather(ctx.handle, ptr(prev), self.N, ptr(self.A), self.N, 1, ptr(out)))
+        return out
+
+    @property
+    def wgts(self):
+        return rs.Weights(lw=self._buf["lw"][self._i, :self.N])
+
+    @property
+    def aux(self):
+        return self.wgts
+
+    @property
+    def W(self):
+        return self.wgts.W
+
+    def __str__(self):
+        return self.fk.summary_format(self)
+
+
+def plan_group(key, R, tier="auto"):
+    """(tier, grid) that ``smcb_batch_plan`` chooses for R runs of the group ``key``."""
+    model, fkind, scheme, N, T = key[:5]
+    d = _lib.BatchDesc()
+    d.model, d.fk, d.scheme, d.dim, d.dy = model, fkind, _lib.RS_CODES[scheme], 1, 1
+    d.tier = {"auto": _lib.BATCH_AUTO, "resident": _lib.BATCH_RESIDENT, "streaming": _lib.BATCH_STREAMING}[tier]
+    d.N, d.T, d.R = N, T, R
+    plan = (C.c_int64 * 2)()
+    ctx = context()
+    _lib.check(ctx.lib.smcb_batch_plan(ctx.handle, C.byref(d), plan))
+    return int(plan[0]), int(plan[1])
+
+
+def run_batch(kws, seeds, noise=None, tier="auto", timer=None, out_func=None, _planned=None):
+    """Run the filters ``SMC(**kws[i], seed=seeds[i])`` -- which must share one ``batch_key`` -- in batched launches
+    and return, per run, its ``BatchRun`` or, with ``out_func``, ``out_func(run)``.
+
+    Memory: the group is cut into chunks that fit half of the free device memory, one launch each.  The streaming
+    tier's CDF and spacings are one scratch set, reused by every chunk and released on return.  With ``out_func`` a
+    chunk's buffers are released as soon as its runs are reduced, so the device holds one chunk at a time; without
+    it every run's outputs stay alive, and each chunk is sized from the memory left after the previous ones.
+    ``noise``: None or one ``(z, u)`` per run with the layout of ``SMC(noise=...)``; ``tier``: "auto", "resident" or
+    "streaming"; ``timer``: None, or a list that receives the pair of CUDA events recorded before the first and
+    after the last launch."""
+    key, specs = _planned or (None, [])
+    if _planned is None:
+        keyed = [batch_key(kw) for kw in kws]
+        keys = {k for k, _ in keyed}
+        if len(keys) != 1 or None in keys:
+            raise ValueError("run_batch: the runs do not form one batchable group")
+        key, specs = keys.pop(), [s for _, s in keyed]
+    model, fkind, scheme, N, T, moments, off = key
+    R, ld = len(kws), N + (N & 1)
+    ctx = context()
+    ctx.bind_stream()
+    dev = ctx.device
+    f64 = dict(dtype=torch.float64, device=dev)
+    n_params = len(specs[0]["params"])
+    d = _lib.BatchDesc()
+    d.model, d.fk, d.scheme, d.dim, d.dy, d.n_params = model, fkind, _lib.RS_CODES[scheme], 1, 1, n_params
+    d.tier = {"auto": _lib.BATCH_AUTO, "resident": _lib.BATCH_RESIDENT, "streaming": _lib.BATCH_STREAMING}[tier]
+    d.N, d.T, d.R = N, T, R
+    plan = (C.c_int64 * 2)()
+    _lib.check(ctx.lib.smcb_batch_plan(ctx.handle, C.byref(d), plan))
+    streaming = plan[0] == _lib.BATCH_STREAMING
+    multi = scheme == "multinomial"
+    # bytes per run: outputs (X ping-pong, lw, A, summary and moment rows) and inputs (data, step constants, params,
+    # seed, ESSrmin, injected noise); the streaming tier's scratch (CDF, spacings) separately
+    noise_b = 0 if noise is None else 8 * T * (N + N + 1)
+    out_b = 8 * (4 * ld + T * (_lib.SUMMARY_STRIDE + (8 if moments else 0) + 2) + n_params + 2) + noise_b
+    scr_b = 8 * (ld + (ld + 2 if multi else 0)) if streaming else 0
+    chunk = max(1, min(R, int(0.5 * torch.cuda.mem_get_info(dev)[0]) // (out_b + scr_b)))
+    scr = None
+    if streaming:
+        scr = {"cdf": torch.empty((chunk, ld), **f64)}
+        if multi:
+            scr["scratch"] = torch.empty((chunk, ld + 2), **f64)
+    ev = None
+    if timer is not None:
+        ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+    out = []
+    r0 = 0
+    while r0 < R:
+        if r0 > 0 and out_func is None:       # earlier chunks stay alive: size this one from what they left
+            chunk = max(1, min(chunk, int(0.5 * torch.cuda.mem_get_info(dev)[0]) // out_b))
+        rc = min(chunk, R - r0)
+        t0 = time.perf_counter()
+        sl = slice(r0, r0 + rc)
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)    # noqa: E731
+        params = up(np.array([np.asarray(s["params"], dtype=np.float64) for s in specs[sl]]))
+        data = up(np.stack([s["data"].reshape(-1) for s in specs[sl]]).astype(np.float64))
+        sc = None
+        if specs[0].get("step_consts") is not None:
+            sc = up(np.stack([np.asarray(s["step_consts"], dtype=np.float64) for s in specs[sl]]))
+        seed_t = up(np.asarray([int(s) & (2 ** 64 - 1) for s in seeds[sl]], dtype=np.uint64).view(np.int64))
+        ess_t = up(np.asarray([float(kw.get("ESSrmin", 0.5)) for kw in kws[sl]], dtype=np.float64))
+        z_t = u_t = None
+        if noise is not None:
+            z_t = as_device(np.stack([np.asarray(z, dtype=np.float64).reshape(T, -1, N) for z, _ in noise[sl]]))
+            u_t = as_device(np.stack([np.asarray(u, dtype=np.float64).reshape(T, N + 1) for _, u in noise[sl]]))
+        b = {"X": torch.empty((rc, 2, ld), **f64), "lw": torch.empty((rc, ld), **f64),
+             "A": torch.empty((rc, ld), dtype=torch.int64, device=dev)}
+        summ = torch.zeros((rc, T, _lib.SUMMARY_STRIDE), **f64)
+        mom = torch.zeros((rc, T, 8), **f64) if moments else None
+        d.R = rc
+        d.seed, d.essrmin, d.params, d.data = seed_t.data_ptr(), ess_t.data_ptr(), params.data_ptr(), data.data_ptr()
+        d.step_consts = None if sc is None else sc.data_ptr()
+        d.X, d.lw, d.A = b["X"].data_ptr(), b["lw"].data_ptr(), b["A"].data_ptr()
+        d.cdf = scr["cdf"].data_ptr() if streaming else None
+        d.scratch = scr["scratch"].data_ptr() if streaming and multi else None
+        d.summaries = summ.data_ptr()
+        d.moments = None if mom is None else mom.data_ptr()
+        d.z_in = None if z_t is None else z_t.data_ptr()
+        d.u_in = None if u_t is None else u_t.data_ptr()
+        if ev is not None and r0 == 0:
+            ev[0].record()
+        _lib.check(ctx.lib.smcb_batch_run(ctx.handle, C.byref(d)))
+        if ev is not None and r0 + rc == R:
+            ev[1].record()
+        table = summ.cpu().numpy()            # the one device->host read of the chunk (+ the moments table)
+        mtab = None if mom is None else mom.cpu().numpy()
+        cpu = (time.perf_counter() - t0) / rc
+        for j in range(rc):
+            kw = kws[r0 + j]
+            run = BatchRun(b, j, kw["fk"], N, scheme, float(kw.get("ESSrmin", 0.5)), seeds[r0 + j], table[j],
+                           None if mtab is None else mtab[j], kw.get("collect"), cpu)
+            out.append(run if out_func is None else out_func(run))
+        del b, run                            # with out_func, nothing refers to this chunk's buffers any more
+        r0 += rc
+    if ev is not None:
+        timer.append(ev)
+    return out
+
+
+def multiSMC(nruns=10, nprocs=0, out_func=None, collect=None, **args):
+    """Run many SMC filters -- ``nruns`` per combination of the list- and dict-valued arguments -- as
+    ``particles.multiSMC`` does (particles/core.py:431-518): same cartesian product, same output dicts (``'run'``,
+    the varied arguments, ``'seed'``, ``'output'``), same seeds after ``np.random.seed``; ``collect`` is never part
+    of the product.  ``'output'`` is ``out_func(run)``, or the run itself (merged into the dict when ``out_func``
+    returns a dict).  As in the reference, ``out_func`` reduces each run as soon as it is done, so only what it
+    returns is kept.
+
+    On the device, a run's seed is its Philox key: output i is the run ``SMC(**args_i, seed=seed_i).run()``, up to
+    the order of floating-point reductions.  Runs that share a model, Feynman-Kac kind, scheme, N, T and collectors
+    form a group (``batch_key``); a group for which ``batch_pays`` holds goes through batched launches
+    (csrc/smcb_batch.cu, one CTA per filter) and its runs are ``BatchRun`` objects.  Every other run goes one by one
+    through ``SMC``.  ``nprocs`` is accepted and has no effect: the device is the parallelism."""
+    from . import utils
+    inputs, outputs = utils.expand(nruns=nruns, seeding=True, protected_args={"collect": collect}, **args)
+    results = [None] * len(inputs)
+    groups, single, specs = {}, [], {}
+    for i, ip in enumerate(inputs):
+        kw = {k: v for k, v in ip.items() if k != "seed"}
+        key, spec = batch_key(kw, specs)
+        if key is None:
+            single.append(i)
+        else:
+            groups.setdefault(key, []).append((i, kw, spec))
+    for key, members in groups.items():
+        n_sm = torch.cuda.get_device_properties(context().device).multi_processor_count
+        if not batch_pays(key[3], len(members), *plan_group(key, len(members)), n_sm=n_sm):
+            single.extend(i for i, _, _ in members)
+            continue
+        outs = run_batch([kw for _, kw, _ in members], [inputs[i]["seed"] for i, _, _ in members],
+                         out_func=out_func, _planned=(key, [spec for _, _, spec in members]))
+        for (i, _, _), o in zip(members, outs):
+            results[i] = o
+    for i in sorted(single):
+        kw = dict(inputs[i])
+        seed = kw.pop("seed")
+        if seed:
+            np.random.seed(seed)                # what the reference's seeder does before each run
+        pf = SMC(seed=int(seed), **kw)
+        pf.run()
+        results[i] = pf if out_func is None else out_func(pf)
+        del pf
+    return [utils.add_to_dict(op, res) for op, res in zip(outputs, results)]

@@ -259,7 +259,7 @@ namespace smcb {
 // workspace layout (doubles): [0, kWsPartials) block partials | 16 scalars | two scan slots
 constexpr size_t kWsPartials = 65536;
 constexpr size_t kWsBytes = 8u << 20;  // 8 MiB: partials + up to ~1M scan tiles
-inline Philox key_of(uint64_t seed) {
+__host__ __device__ inline Philox key_of(uint64_t seed) {
     Philox k;
     k.k0 = (uint32_t)seed;
     k.k1 = (uint32_t)(seed >> 32);

@@ -55,7 +55,7 @@ struct StochVolM {
     static constexpr int D = 1, NZ = 1;   // state dimension, normals per particle
     double mu, rho, sigma, sig0, c0, lsigma, lsig0;
     static constexpr bool has_proposal = true;
-    __host__ void load(const double *p) {
+    __host__ __device__ void load(const double *p) {
         mu = p[0]; rho = p[1]; sigma = p[2]; sig0 = p[3]; c0 = p[4]; lsigma = p[5]; lsig0 = p[6];
     }
     __device__ __forceinline__ void init(double &loc, double &scale, double &ls) const {
@@ -104,7 +104,7 @@ struct LinGaussM {
     static constexpr int D = 1, NZ = 1;   // state dimension, normals per particle
     double rho, sX, sY, s0, lsX, lsY, ls0, s2p0, sp0, lsp0, s2p, sp, lsp, se, lse, sX2, sY2;
     static constexpr bool has_proposal = true;
-    __host__ void load(const double *p) {
+    __host__ __device__ void load(const double *p) {
         rho = p[0]; sX = p[1]; sY = p[2]; s0 = p[3]; lsX = p[4]; lsY = p[5]; ls0 = p[6];
         s2p0 = p[7]; sp0 = p[8]; lsp0 = p[9]; s2p = p[10]; sp = p[11]; lsp = p[12];
         se = p[13]; lse = p[14]; sX2 = p[15]; sY2 = p[16];
@@ -139,7 +139,7 @@ struct GordonM {
     static constexpr int D = 1, NZ = 1;   // state dimension, normals per particle
     double a, b, c, sX, lsX;
     static constexpr bool has_proposal = false;
-    __host__ void load(const double *p) { a = p[0]; b = p[1]; c = p[2]; sX = p[3]; lsX = p[4]; }
+    __host__ __device__ void load(const double *p) { a = p[0]; b = p[1]; c = p[2]; sX = p[3]; lsX = p[4]; }
     __device__ __forceinline__ void init(double &loc, double &scale, double &ls) const {
         loc = 0.0; scale = 2.0; ls = 0.69314718055994530942;      // Normal(scale=2.), :563-564
     }
@@ -164,7 +164,7 @@ struct ThetaLogisticM {
     static constexpr int D = 1, NZ = 1;   // state dimension, normals per particle
     double tau0, tau1, tau2, sX, sY, lsX, lsY;
     static constexpr bool has_proposal = false;
-    __host__ void load(const double *p) {
+    __host__ __device__ void load(const double *p) {
         tau0 = p[0]; tau1 = p[1]; tau2 = p[2]; sX = p[3]; sY = p[4]; lsX = p[5]; lsY = p[6];
     }
     __device__ __forceinline__ void init(double &loc, double &scale, double &ls) const {
@@ -191,7 +191,7 @@ struct StochVolLevM {
     static constexpr int D = 1, NZ = 1;
     static constexpr bool has_proposal = false;
     double mu, rho, sigma, sig0, c0, lsigma, lsig0, phi, sq, lsq;
-    __host__ void load(const double *p) {
+    __host__ __device__ void load(const double *p) {
         mu = p[0]; rho = p[1]; sigma = p[2]; sig0 = p[3]; c0 = p[4]; lsigma = p[5]; lsig0 = p[6];
         phi = p[7]; sq = p[8]; lsq = p[9];
     }
@@ -223,7 +223,7 @@ struct DiscreteCoxM {
     static constexpr int D = 1, NZ = 1;
     static constexpr bool has_proposal = false;
     double mu, sigma, phi, sig0, lsigma, lsig0;
-    __host__ void load(const double *p) {
+    __host__ __device__ void load(const double *p) {
         mu = p[0]; sigma = p[1]; phi = p[2]; sig0 = p[3]; lsigma = p[4]; lsig0 = p[5];
     }
     __device__ __forceinline__ void init(double &loc, double &scale, double &ls) const {
@@ -302,7 +302,7 @@ struct BearingsM {
     static constexpr int D = 4, NZ = 2;
     static constexpr bool has_proposal = false;
     double sX, sY, lsY, x0[4], lsX, isX;
-    __host__ void load(const double *p) {
+    __host__ __device__ void load(const double *p) {
         sX = p[0]; sY = p[1]; lsY = p[2];
         for (int i = 0; i < 4; i++) x0[i] = p[3 + i];
         lsX = p[7]; isX = 1.0 / sX;
@@ -356,7 +356,7 @@ struct MvLinGaussM {
     // x / c = fma(fma(-q, c, x), r, q) with q = x * r, r = RN(1 / c) is the correctly rounded quotient (Markstein) in 3
     // instructions instead of the ~20-instruction division sequence with its slow-path call
     double iLX[DX], iLY[kMaxDy], iLP[DX], iLE[kMaxDy], iL0[DX], iLP0[DX];
-    __host__ void load(const double *p) {
+    __host__ __device__ void load(const double *p) {
         dy = (int)p[0]; p += 1;
         auto take = [&](double *dst, int cnt) { for (int i = 0; i < cnt; i++) dst[i] = p[i]; p += cnt; };
         take(F, DX * DX); take(G, kMaxDy * DX); take(LX, DX * DX); take(&hldX, 1);
