@@ -119,20 +119,16 @@ __global__ void __launch_bounds__(kBatchBS) k_batch(const smcb_batch_desc d, con
                 scan_range<BS>(load, 0, n, 0.0, CUDART_INF, cdf, s_warp);
                 if (MULTI) {                             // exponential spacings, n + 1 of them (resampling.py:536-537)
                     for (int64_t i = 2 * (int64_t)threadIdx.x; i <= n; i += 2 * BS) {
-                        double u0, u1;
-                        if (ut) { u0 = ut[i]; u1 = (i + 1 <= n) ? ut[i + 1] : 1.0; }
-                        else uniform_pair(key, (uint64_t)(i >> 1), (uint32_t)t, kPurposeUniform, u0, u1);
-                        su[i] = -log(u0);                // u may be 0 or injected: library log
-                        if (i + 1 <= n) su[i + 1] = -log(u1);
+                        double v0, v1;
+                        spacings_pair(key, (uint32_t)t, ut, i, n + 1, v0, v1);
+                        su[i] = v0;
+                        if (i + 1 <= n) su[i + 1] = v1;
                     }
                     __syncthreads();
                     scan_range<BS>(LoadPlain{su}, 0, n + 1, 0.0, CUDART_INF, su, s_warp);
                     zlast = su[n];
                 }
-                if (SCHEME == SMCB_RS_SYSTEMATIC) {
-                    if (ut) u_sys = ut[0];
-                    else { double u1; uniform_pair(key, 0ull, (uint32_t)t, kPurposeUniform, u_sys, u1); }
-                }
+                if (SCHEME == SMCB_RS_SYSTEMATIC) u_sys = systematic_u(key, t, ut);
             }
             const bool last_apf = APF && t + 1 < T;
             const bool write_A = rs && t == T - 1;
@@ -142,11 +138,7 @@ __global__ void __launch_bounds__(kBatchBS) k_batch(const smcb_batch_desc d, con
             for (int64_t p = threadIdx.x; p < npairs; p += BS) {
                 const bool two = 2 * p + 1 < n;
                 double z[2][NZ];
-#pragma unroll
-                for (int c = 0; c < NZ; c++) {
-                    if (zt) { z[0][c] = zt[c * n + 2 * p]; z[1][c] = two ? zt[c * n + 2 * p + 1] : 0.0; }
-                    else normal_pair_tab(key, (uint64_t)p, (uint32_t)t, (uint32_t)c, z[0][c], z[1][c]);
-                }
+                pair_normals<NZ>(key, (uint64_t)p, (uint32_t)t, zt, n, p, z);
                 double x[2][1], l[2], av[2];
                 if (t == 0) {                            // generate_particles + reweight (core.py:315-324)
 #pragma unroll

@@ -705,6 +705,80 @@ __device__ __forceinline__ void cta_range(const FilterArgs &a, int64_t &pstart, 
 }
 
 // ---------------------------------------------------------------------------
+// one pair of particles 2p, 2p + 1: the pair is the unit of the Philox normals and of the paired stores.  k_batch
+// (smcb_batch.cu) draws its normals through pair_normals too, so a batched run draws what the single filter draws.
+// ---------------------------------------------------------------------------
+// the normals of the pair at step t: the table-family Box-Muller of Philox pair counter `pair` ...
+template <int NZ>
+__device__ __forceinline__ void tab_normals(const Philox &key, uint64_t pair, uint32_t t, double (&z)[2][NZ]) {
+#pragma unroll
+    for (int c = 0; c < NZ; c++) normal_pair_tab(key, pair, t, (uint32_t)c, z[0][c], z[1][c]);
+}
+// ... or those of the step's injected (NZ, n) slice zin if it is not NULL; an absent second particle (2p + 1 = n) gets 0
+template <int NZ>
+__device__ __forceinline__ void pair_normals(const Philox &key, uint64_t pair, uint32_t t, const double *zin, int64_t n,
+                                             int64_t p, double (&z)[2][NZ]) {
+    if (!zin) return tab_normals<NZ>(key, pair, t, z);
+#pragma unroll
+    for (int c = 0; c < NZ; c++) {
+        z[0][c] = zin[(size_t)c * n + 2 * p];
+        z[1][c] = (2 * p + 1 < n) ? zin[(size_t)c * n + 2 * p + 1] : 0.0;
+    }
+}
+
+// propagate the pair from xp (INIT: generate it; core.py:315-324) and weight it: lw = base + logG (Weights.add,
+// resampling.py:241-244; INIT: lw = logG), and for an APF whose step t + 1 exists (`next`) the auxiliary weight
+// lw + logeta_t(x).  NaN -> -inf (resampling.py:220).  Returns whether any of these values was +-inf / NaN (integer
+// test), so that a caller can accumulate a finite batch with acc_add_batch's FINITE case.
+template <class M, int FK, bool INIT>
+__device__ __forceinline__ bool move_pair(const M &model, const StepK &k, const double (*xp)[M::D], const double *base,
+                                          const double (&z)[2][M::NZ], bool next, double (&x)[2][M::D], double *l,
+                                          double *av) {
+    constexpr bool APF = FkTraits<FK>::apf;
+    bool odd = false;
+#pragma unroll
+    for (int j = 0; j < 2; j++) {
+        double d;
+        if (INIT) model_init<M, FK>(model, k, z[j], x[j], d);
+        else model_move<M, FK>(model, k, xp[j], z[j], x[j], d);
+        l[j] = INIT ? d : base[j] + d;
+        odd |= nonfinite(l[j]);
+        if (APF) {
+            av[j] = next ? l[j] + model_logeta<M>(model, k, x[j]) : -CUDART_INF;
+            odd |= nonfinite(av[j]);
+        }
+    }
+    if (odd) {
+#pragma unroll
+        for (int j = 0; j < 2; j++) { l[j] = fix_nan(l[j]); if (APF) av[j] = fix_nan(av[j]); }
+    }
+    return odd;
+}
+
+// store the pair into SoA buffers of n particles (component stride n).  An odd n's last particle is stored alone, and
+// its partner slot is masked (x = 0, lw = av = -inf) so that it contributes exactly 0 to the accumulators.
+template <int D, bool APF>
+__device__ __forceinline__ void store_pair(double *Xo, double *lwo, int64_t n, int64_t p, bool vec_x, double (&x)[2][D],
+                                           double *l, double *av) {
+    if (2 * p + 1 < n) {
+        if (vec_x) {
+#pragma unroll
+            for (int c = 0; c < D; c++) st2(Xo + (size_t)c * n + 2 * p, x[0][c], x[1][c]);
+        } else {                                      // odd SoA stride: component rows are only 8-byte aligned
+#pragma unroll
+            for (int c = 0; c < D; c++) { Xo[(size_t)c * n + 2 * p] = x[0][c]; Xo[(size_t)c * n + 2 * p + 1] = x[1][c]; }
+        }
+        st2(lwo + 2 * p, l[0], l[1]);
+    } else {
+#pragma unroll
+        for (int c = 0; c < D; c++) { Xo[(size_t)c * n + 2 * p] = x[0][c]; x[1][c] = 0.0; }
+        lwo[2 * p] = l[0];
+        l[1] = -CUDART_INF;
+        if (APF) av[1] = -CUDART_INF;
+    }
+}
+
+// ---------------------------------------------------------------------------
 // t = 0: generate_particles + reweight (core.py:315-324, 373-374)
 // ---------------------------------------------------------------------------
 template <class M, int FK>
@@ -729,38 +803,9 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_init(M model, FilterArgs 
     cta_range(a, pstart, pend);
     for (int64_t p = pstart + threadIdx.x; p < pend; p += BS) {
         double z[2][NZ], x[2][D], l[2], av[2];
-#pragma unroll
-        for (int c = 0; c < NZ; c++) {
-            if (a.z_in) {                                  // injected normals: (T, NZ, n)
-                const double *zz = a.z_in + (size_t)c * n;
-                z[0][c] = zz[2 * p];
-                z[1][c] = (2 * p + 1 < n) ? zz[2 * p + 1] : 0.0;
-            } else {
-                normal_pair_tab(a.key, (uint64_t)((a.index_offset >> 1) + p), 0u, (uint32_t)c, z[0][c], z[1][c]);
-            }
-        }
-#pragma unroll
-        for (int j = 0; j < 2; j++) {
-            double d;
-            model_init<M, FK>(model, k, z[j], x[j], d);
-            l[j] = fix_nan(d);
-            av[j] = has_next ? fix_nan(l[j] + model_logeta<M>(model, k, x[j])) : -CUDART_INF;
-        }
-        if (2 * p + 1 < n) {
-            if (vec_x) {
-#pragma unroll
-                for (int c = 0; c < D; c++) st2(Xo + (size_t)c * n + 2 * p, x[0][c], x[1][c]);
-            } else {                                      // odd SoA stride: component rows are only 8-byte aligned
-#pragma unroll
-                for (int c = 0; c < D; c++) { Xo[(size_t)c * n + 2 * p] = x[0][c]; Xo[(size_t)c * n + 2 * p + 1] = x[1][c]; }
-            }
-            st2(lwo + 2 * p, l[0], l[1]);
-        } else {
-#pragma unroll
-            for (int c = 0; c < D; c++) { Xo[(size_t)c * n + 2 * p] = x[0][c]; x[1][c] = 0.0; }
-            lwo[2 * p] = l[0];
-            l[1] = -CUDART_INF; av[1] = -CUDART_INF;   // masked slot contributes exactly 0
-        }
+        pair_normals<NZ>(a.key, (uint64_t)((a.index_offset >> 1) + p), 0u, a.z_in, n, p, z);
+        move_pair<M, FK, true>(model, k, nullptr, nullptr, z, has_next, x, l, av);
+        store_pair<D, APF>(Xo, lwo, n, p, vec_x, x, l, av);
         acc_add_batch<2, D>(acc, l, x, mom);
         if (APF) lse3_add_batch<2>(aux, av);
     }
@@ -1043,6 +1088,46 @@ __device__ __forceinline__ void scan_scatter_groups(const LOAD &load, int64_t e0
     __syncthreads();
 }
 
+// ---------------------------------------------------------------------------
+// grid points.  Uniforms: injected row uin = (n + 1) of the step, or Philox (purpose kPurposeUniform, pair index, t).
+// ---------------------------------------------------------------------------
+// systematic resampling's one uniform of step t (resampling.py:609)
+__device__ __forceinline__ double systematic_u(const Philox &key, long long t, const double *uin) {
+    if (uin) return uin[0];
+    double u0, u1;
+    uniform_pair(key, 0ull, (uint32_t)t, kPurposeUniform, u0, u1);
+    return u0;
+}
+
+// su_k of the outputs 2p, 2p + 1 of pair p out of M: systematic (u_sys + k) / M (resampling.py:609) or stratified
+// (u_k + k) / M (resampling.py:602) with the uniforms of Philox pair `pair`.  Stratified draws only for a `valid` pair;
+// an absent second output (!two) gets u = 0.
+template <int SCHEME>
+__device__ __forceinline__ void grid_pair(double u_sys, const Philox &key, uint64_t pair, uint32_t t, const double *uin,
+                                          int64_t p, bool valid, bool two, double M, double &su0, double &su1) {
+    double u0 = u_sys, u1 = u_sys;
+    if (SCHEME == SMCB_RS_STRATIFIED) {
+        u0 = 0.0; u1 = 0.0;
+        if (valid) {
+            if (uin) { u0 = uin[2 * p]; u1 = two ? uin[2 * p + 1] : 0.0; }
+            else uniform_pair(key, pair, t, kPurposeUniform, u0, u1);
+        }
+    }
+    su0 = (u0 + (double)(2 * p)) / M;
+    su1 = (u1 + (double)(2 * p + 1)) / M;
+}
+
+// multinomial: the exponential spacings -log u_i, -log u_{i+1} (resampling.py:536-537) for even i; entry i + 1
+// exists if i + 1 < e, else it is 0
+__device__ __forceinline__ void spacings_pair(const Philox &key, uint32_t t, const double *uin, int64_t i, int64_t e,
+                                              double &v0, double &v1) {
+    double u0, u1;
+    if (uin) { u0 = uin[i]; u1 = (i + 1 < e) ? uin[i + 1] : 1.0; }
+    else uniform_pair(key, (uint64_t)(i >> 1), t, kPurposeUniform, u0, u1);
+    v0 = -log(u0);                    // u may be 0 or injected: library log
+    v1 = (i + 1 < e) ? -log(u1) : 0.0;
+}
+
 // multinomial: exponential spacings z = cumsum(-log u), n + 1 of them (resampling.py:536-537), blocked like
 // the weights: pass 1 leaves v_i = -log u_i in su[] and the CTA's sum in blk_agg[]; after a grid barrier
 // pass 2 scans the CTA's range from the (fixed-order, monotone) prefix of the CTA sums.
@@ -1069,11 +1154,8 @@ __device__ __forceinline__ void spacings_pass1(const FilterArgs &a, long long t,
     const double *uin = a.u_in ? a.u_in + (size_t)t * (a.n + 1) : nullptr;
     double acc[1] = {0.0};
     for (int64_t i = e0 + 2 * (int64_t)threadIdx.x; i < e1; i += 2 * BS) {
-        double u0, u1;
-        if (uin) { u0 = uin[i]; u1 = (i + 1 < e1) ? uin[i + 1] : 1.0; }
-        else uniform_pair(a.key, (uint64_t)(i >> 1), (uint32_t)t, kPurposeUniform, u0, u1);
-        const double v0 = -log(u0);                    // u may be 0 or injected: library log
-        const double v1 = (i + 1 < e1) ? -log(u1) : 0.0;
+        double v0, v1;
+        spacings_pair(a.key, (uint32_t)t, uin, i, e1, v0, v1);
         a.su[i] = v0;
         if (i + 1 < e1) a.su[i + 1] = v1;
         acc[0] += v0 + v1;
@@ -1206,40 +1288,9 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
     auto do_pair = [&](const StepIo &io, int64_t p, const double (&xp)[2][D], const double (&base)[2],
                        double (&x)[2][D], double *l, double *av) {
         double z[2][NZ];
-#pragma unroll
-        for (int c = 0; c < NZ; c++) {
-            if (io.zin) {                                // injected normals: (T, NZ, n)
-                const double *zz = io.zin + (size_t)c * n;
-                z[0][c] = zz[2 * p];
-                z[1][c] = (2 * p + 1 < n) ? zz[2 * p + 1] : 0.0;
-            } else {
-                normal_pair_tab(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)io.t, (uint32_t)c,
-                                 z[0][c], z[1][c]);
-            }
-        }
-#pragma unroll
-        for (int j = 0; j < 2; j++) {
-            double d;
-            model_move<M, FK>(model, io.k, xp[j], z[j], x[j], d);
-            l[j] = fix_nan(base[j] + d);                          // Weights.add, resampling.py:241-244
-            if (APF) av[j] = io.last_apf ? fix_nan(l[j] + model_logeta<M>(model, io.k, x[j])) : -CUDART_INF;
-        }
-        if (2 * p + 1 < n) {
-            if (vec_x) {
-#pragma unroll
-                for (int c = 0; c < D; c++) st2(io.Xo + (size_t)c * n + 2 * p, x[0][c], x[1][c]);
-            } else {
-#pragma unroll
-                for (int c = 0; c < D; c++) { io.Xo[(size_t)c * n + 2 * p] = x[0][c]; io.Xo[(size_t)c * n + 2 * p + 1] = x[1][c]; }
-            }
-            st2(io.lwo + 2 * p, l[0], l[1]);
-        } else {
-#pragma unroll
-            for (int c = 0; c < D; c++) { io.Xo[(size_t)c * n + 2 * p] = x[0][c]; x[1][c] = 0.0; }
-            io.lwo[2 * p] = l[0];
-            l[1] = -CUDART_INF;
-            if (APF) av[1] = -CUDART_INF;
-        }
+        pair_normals<NZ>(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)io.t, io.zin, n, p, z);
+        move_pair<M, FK, false>(model, io.k, xp, base, z, io.last_apf, x, l, av);
+        store_pair<D, APF>(io.Xo, io.lwo, n, p, vec_x, x, l, av);
     };
 
     if (!rs) {
@@ -1282,9 +1333,9 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
             for (int u = 0; u < kU; u++) {
                 const int prel = i * kIt + u * 32 + lane;
                 double z[2][NZ];
-#pragma unroll
-                for (int c = 0; c < NZ; c++)
-                    normal_pair_tab(a.key, gpair0 + (uint64_t)prel, (uint32_t)io.t, (uint32_t)c, z[0][c], z[1][c]);
+                tab_normals<NZ>(a.key, gpair0 + (uint64_t)prel, (uint32_t)io.t, z);
+                // (move_pair's arithmetic written out: this is the streaming pass's inner loop, and it takes one NaN
+                // fix-up per iteration instead of one per pair)
 #pragma unroll
                 for (int j2 = 0; j2 < 2; j2++) {
                     double d;
@@ -1492,11 +1543,7 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
         constexpr int kBarriers = (SCHEME == SMCB_RS_MULTINOMIAL) ? 2 : 1;     // grid barriers per resampling step
         unsigned long long bar_target = (unsigned long long)gridDim.x * ((unsigned long long)dec.nrs_prev * kBarriers);
         const double *uin = a.u_in ? a.u_in + (size_t)t * (n + 1) : nullptr;
-        double u_sys = 0.0;
-        if (SCHEME == SMCB_RS_SYSTEMATIC) {
-            if (uin) u_sys = uin[0];
-            else { double u1; uniform_pair(a.key, 0ull, (uint32_t)t, kPurposeUniform, u_sys, u1); }
-        }
+        const double u_sys = (SCHEME == SMCB_RS_SYSTEMATIC) ? systematic_u(a.key, t, uin) : 0.0;
         constexpr bool kCount = (SCHEME != SMCB_RS_MULTINOMIAL);      // offspring counting (local resampling only)
         const bool count_path = kCount && !a.rs_global;
         {
@@ -1549,25 +1596,8 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
             double l[2], av[2];
             if (zin == nullptr && vec_x && 2 * p + 1 < n) {       // complete pair, device normals: no bounds tests
                 double z[2][NZ];
-#pragma unroll
-                for (int c = 0; c < NZ; c++)
-                    normal_pair_tab(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t, (uint32_t)c, z[0][c], z[1][c]);
-                bool odd = false;
-#pragma unroll
-                for (int j2 = 0; j2 < 2; j2++) {
-                    double d;
-                    model_move<M, FK>(model, k, xp[j2], z[j2], x[j2], d);
-                    l[j2] = base[j2] + d;
-                    odd |= nonfinite(l[j2]);
-                    if (APF) {
-                        av[j2] = last_apf ? l[j2] + model_logeta<M>(model, k, x[j2]) : -CUDART_INF;
-                        odd |= nonfinite(av[j2]);
-                    }
-                }
-                if (odd) {
-#pragma unroll
-                    for (int j2 = 0; j2 < 2; j2++) { l[j2] = fix_nan(l[j2]); if (APF) av[j2] = fix_nan(av[j2]); }
-                }
+                tab_normals<NZ>(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t, z);
+                const bool odd = move_pair<M, FK, false>(model, k, xp, base, z, last_apf, x, l, av);
 #pragma unroll
                 for (int c = 0; c < D; c++) st2(Xo + (size_t)c * n + 2 * p, x[0][c], x[1][c]);
                 st2(lwo + 2 * p, l[0], l[1]);
@@ -1654,18 +1684,8 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
                     moved[r] = false;
                     valid[r] = p < pend;
                     two[r] = valid[r] && (2 * p + 1 < n);
-                    if (SCHEME == SMCB_RS_SYSTEMATIC) {                    // resampling.py:609
-                        su[r][0] = (u_sys + (double)(2 * p)) / M_;
-                        su[r][1] = (u_sys + (double)(2 * p + 1)) / M_;
-                    } else {                                               // resampling.py:602
-                        double u0 = 0.0, u1 = 0.0;
-                        if (valid[r]) {
-                            if (uin) { u0 = uin[2 * p]; u1 = two[r] ? uin[2 * p + 1] : 0.0; }
-                            else uniform_pair(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t, kPurposeUniform, u0, u1);
-                        }
-                        su[r][0] = (u0 + (double)(2 * p)) / M_;
-                        su[r][1] = (u1 + (double)(2 * p + 1)) / M_;
-                    }
+                    grid_pair<SCHEME>(u_sys, a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t, uin, p, valid[r],
+                                      two[r], M_, su[r][0], su[r][1]);
 #pragma unroll
                     for (int q = 0; q < 2; q++) {
                         long long hh = H.h[r][q];
@@ -1723,9 +1743,9 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
                 ld_cdf(p0, H, Cc);
                 process(p0, H, Cc);
             }
-        } else if (!a.rs_global) {
-            const double M_ = (double)n;
-            const double zlast = (SCHEME == SMCB_RS_MULTINOMIAL) ? __ldcg(a.su + n) : 1.0;
+        } else if (SCHEME == SMCB_RS_MULTINOMIAL && !a.rs_global) {
+            // (every other scheme counts offspring when it resamples locally)
+            const double zlast = __ldcg(a.su + n);
             int64_t lo = -1;
             if (threadIdx.x == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_init_fence(); }
             __syncthreads();
@@ -1755,20 +1775,8 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
                 const int64_t k1 = (2 * ptop < n ? 2 * ptop : n) - 1;
                 double su[2] = {2.0, 2.0};
                 if (active) {
-                    if (SCHEME == SMCB_RS_SYSTEMATIC) {                    // resampling.py:609
-                        su[0] = (u_sys + (double)(2 * p)) / M_;
-                        su[1] = (u_sys + (double)(2 * p + 1)) / M_;
-                    } else if (SCHEME == SMCB_RS_STRATIFIED) {             // resampling.py:602
-                        double u0, u1;
-                        if (uin) { u0 = uin[2 * p]; u1 = (2 * p + 1 < n) ? uin[2 * p + 1] : 0.0; }
-                        else uniform_pair(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t,
-                                          kPurposeUniform, u0, u1);
-                        su[0] = (u0 + (double)(2 * p)) / M_;
-                        su[1] = (u1 + (double)(2 * p + 1)) / M_;
-                    } else {                                               // resampling.py:537
-                        su[0] = __ldcg(a.su + 2 * p) / zlast;
-                        su[1] = (2 * p + 1 < n) ? __ldcg(a.su + 2 * p + 1) / zlast : 2.0;
-                    }
+                    su[0] = __ldcg(a.su + 2 * p) / zlast;                   // resampling.py:537
+                    su[1] = (2 * p + 1 < n) ? __ldcg(a.su + 2 * p + 1) / zlast : 2.0;
                     if (2 * p == k0) s_su[0] = su[0];
                     if (2 * p == k1) s_su[1] = su[0];
                     if (2 * p + 1 == k1) s_su[1] = su[1];
