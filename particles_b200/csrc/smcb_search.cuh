@@ -2,9 +2,32 @@
 //   A[k] = min{ j : cdf[j] >= su[k] }   == np.searchsorted(cdf, su, side='left'),
 // clipped to n-1 (the numba loop of the reference has no bounds check).
 #pragma once
+#ifndef SMCB_MATH_HOST_TEST      // tests/math_host.cpp compiles tile_search for the CPU with its own shim
 #include "smcb_common.cuh"
+#endif
 
 namespace smcb {
+
+// The search inside a staged CDF tile (the step kernel's multinomial and global-resampling move passes).  s holds
+// cdf[sbase, sbase + cnt); the answers of the tile's outputs are known to lie at or after s[l0] (l0 = lo - sbase).
+// r0, r1 = the first j in [l0, cnt) with s[j] >= v0, v1 (cnt if none) for one output pair, v0 <= v1.
+// v1 lies on average one CDF entry past v0: it walks forward a few entries before it falls back to bisection
+// (same result as searchsorted).
+__device__ __forceinline__ void tile_search(const double *s, int l0, int cnt, double v0, double v1, int &r0, int &r1) {
+    int h0 = cnt;
+    while (l0 < h0) { const int mid = (l0 + h0) >> 1; if (s[mid] < v0) l0 = mid + 1; else h0 = mid; }
+    int l1 = l0, h1 = cnt;
+#pragma unroll
+    for (int w = 0; w < 4; w++)
+        if (l1 < cnt && s[l1] < v1) l1++;
+    if (l1 < cnt && s[l1] < v1) {
+        while (l1 < h1) { const int mid = (l1 + h1) >> 1; if (s[mid] < v1) l1 = mid + 1; else h1 = mid; }
+    }
+    r0 = l0;
+    r1 = l1;
+}
+
+#ifndef SMCB_MATH_HOST_TEST
 
 // first j in [lo, hi) with cdf[j] >= key, hi if none; cdf non-decreasing
 __device__ __forceinline__ int64_t lower_bound(const double *__restrict__ cdf, int64_t lo,
@@ -48,5 +71,7 @@ __device__ __forceinline__ int64_t block_lower_bound(const double *__restrict__ 
     }
     return lo;
 }
+
+#endif
 
 }  // namespace smcb

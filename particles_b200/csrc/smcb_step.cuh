@@ -1203,6 +1203,727 @@ __device__ __forceinline__ StepIo step_io(const FilterArgs &a, long long t, int 
     return io;
 }
 
+// what every phase of one k_step launch reads: step t's constants and output buffers, the step that wrote the input
+// buffers, and this CTA's range of pairs
+struct StepEnv {
+    StepIo io;               // step t
+    StepK kprev;             // step t - 1, whose weights the resampling branch resamples
+    int cur;                 // step t - 1 wrote buffers [cur]
+    int64_t n;
+    int64_t pstart, pend;    // this CTA's pairs
+    bool vec_x;              // SoA component rows are 16-byte aligned
+    bool mom;                // moments are collected
+};
+
+// propagate + reweight one pair of particles by step io.t; writes x', lw'; returns x', lw' (and the auxiliary
+// log-weights of the next step for an APF), -inf in masked slots
+template <class M, int FK>
+__device__ __forceinline__ void do_pair(const M &model, const FilterArgs &a, const StepIo &io, int64_t n, bool vec_x,
+                                        int64_t p, const double (&xp)[2][M::D], const double (&base)[2],
+                                        double (&x)[2][M::D], double *l, double *av) {
+    double z[2][M::NZ];
+    pair_normals<M::NZ>(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)io.t, io.zin, n, p, z);
+    move_pair<M, FK, false>(model, io.k, xp, base, z, io.last_apf, x, l, av);
+    store_pair<M::D, FkTraits<FK>::apf>(io.Xo, io.lwo, n, p, vec_x, x, l, av);
+}
+
+// The streaming pass: A = arange(N), Xp = X (core.py:335-336).  Step t -- FUSED: and step t + 1 -- over this CTA's
+// pairs.  The statistics go to slab records: step t's in s_stage, step t + 1's in the CTA's slice of fuse_slab.
+// Returns the number of records.  Work unit = one "iteration" of a warp: kU x 32 consecutive pairs (kU coalesced
+// 512-byte rows per array), kU pairs in flight per thread.
+template <class M, int FK, bool FUSED>
+__device__ __forceinline__ int stream_pass(const M &model, const FilterArgs &a, const StepEnv &e, StepSmem &sh,
+                                           double *s_stage) {
+    constexpr bool APF = FkTraits<FK>::apf;
+    constexpr int D = M::D, NZ = M::NZ;
+    constexpr int kU = StepCfg<M>::kU;
+    constexpr int kIt = 32 * kU;                                          // pairs per iteration
+    const StepIo &io0 = e.io;
+    const int64_t n = e.n, pstart = e.pstart, pend = e.pend;
+    const bool vec_x = e.vec_x, mom = e.mom;
+    const double *__restrict__ Xi = a.X[e.cur];
+    const double *__restrict__ lwi = a.lw[e.cur];
+    const int lane = threadIdx.x & 31;
+    const int npl = (int)(pend - pstart);                                 // pairs of this CTA (< 2^31)
+    const int n_iter = (npl + kIt - 1) / kIt;
+    // iterations made of complete pairs only run without any bounds test (the odd last particle and the ragged
+    // end of the range take the general path)
+    const int64_t whole = (n >> 1) < pend ? (n >> 1) : pend;
+    const int n_full = whole > pstart ? (int)((whole - pstart) / kIt) : 0;
+    const bool fast_ok = (io0.zin == nullptr) && vec_x;
+    const double *__restrict__ lwi_c = lwi + 2 * pstart;
+    const double *__restrict__ Xi_c = Xi + 2 * pstart;
+    const uint64_t gpair0 = (uint64_t)((a.index_offset >> 1) + pstart);
+    // one iteration: pairs (relative to pstart) i * kIt + u * 32 + lane.  Loads and arithmetic are separate so
+    // that the inputs of the NEXT iteration can be requested before the current one is computed.
+    struct In { double base[kU][2]; double xp[kU][2][D]; };
+    auto load_full = [&](const double *Xs_c, const double *lws_c, int i, In &in) {
+#pragma unroll
+        for (int u = 0; u < kU; u++) {
+            const int o2 = 2 * (i * kIt + u * 32 + lane);
+            const double2 tl = ld2(lws_c + o2);
+            in.base[u][0] = tl.x; in.base[u][1] = tl.y;
+#pragma unroll
+            for (int c = 0; c < D; c++) {
+                const double2 tx = ld2(Xs_c + (size_t)c * n + o2);
+                in.xp[u][0][c] = tx.x; in.xp[u][1][c] = tx.y;
+            }
+        }
+    };
+    auto compute_full = [&](const StepIo &io, int i, const In &in, Acc<D> &ac, Lse3 &ax, double (&l)[2 * kU],
+                            double (&x)[2 * kU][D]) {
+        double av[APF ? 2 * kU : 1];
+        bool odd = false;                                 // some value is +-inf / NaN (integer test)
+#pragma unroll
+        for (int u = 0; u < kU; u++) {
+            const int prel = i * kIt + u * 32 + lane;
+            double z[2][NZ];
+            tab_normals<NZ>(a.key, gpair0 + (uint64_t)prel, (uint32_t)io.t, z);
+            // (move_pair's arithmetic written out: this is the streaming pass's inner loop, and it takes one NaN
+            // fix-up per iteration instead of one per pair)
+#pragma unroll
+            for (int j2 = 0; j2 < 2; j2++) {
+                double d;
+                model_move<M, FK>(model, io.k, in.xp[u][j2], z[j2], x[2 * u + j2], d);
+                l[2 * u + j2] = in.base[u][j2] + d;                   // Weights.add, resampling.py:241-244
+                odd |= nonfinite(l[2 * u + j2]);
+                if (APF) {
+                    av[APF ? 2 * u + j2 : 0] = io.last_apf ? l[2 * u + j2] + model_logeta<M>(model, io.k, x[2 * u + j2])
+                                                           : -CUDART_INF;
+                    odd |= nonfinite(av[APF ? 2 * u + j2 : 0]);
+                }
+            }
+        }
+        if (odd) {                                        // rare: NaN -> -inf (resampling.py:220)
+#pragma unroll
+            for (int q = 0; q < 2 * kU; q++) {
+                l[q] = fix_nan(l[q]);
+                if (APF) av[APF ? q : 0] = fix_nan(av[APF ? q : 0]);
+            }
+        }
+        double *const lwo_c = io.lwo + 2 * pstart;
+        double *const Xo_c = io.Xo + 2 * pstart;
+#pragma unroll
+        for (int u = 0; u < kU; u++) {
+            const int o2 = 2 * (i * kIt + u * 32 + lane);
+#pragma unroll
+            for (int c = 0; c < D; c++) st2(Xo_c + (size_t)c * n + o2, x[2 * u][c], x[2 * u + 1][c]);
+            st2(lwo_c + o2, l[2 * u], l[2 * u + 1]);
+        }
+        if (!odd) {
+            acc_add_batch<2 * kU, D, true>(ac, l, x, mom);
+        } else {
+            acc_add_batch<2 * kU, D, false>(ac, l, x, mom);
+        }
+        if (APF) lse3_add_batch<(APF ? 2 * kU : 1)>(ax, av);
+    };
+    // general path: ragged end of the range, the odd last particle, injected normals, odd SoA stride
+    auto load_general = [&](const double *Xs, const double *lws, int i, In &in) {
+        const int64_t qbase = pstart + (int64_t)i * kIt;
+#pragma unroll
+        for (int u = 0; u < kU; u++) {
+            const int64_t p = qbase + u * 32 + lane;
+            if (p < pend && 2 * p + 1 < n) {
+                double2 tl = ld2(lws + 2 * p);
+                in.base[u][0] = tl.x; in.base[u][1] = tl.y;
+#pragma unroll
+                for (int c = 0; c < D; c++) {
+                    if (vec_x) {
+                        double2 tx = ld2(Xs + (size_t)c * n + 2 * p);
+                        in.xp[u][0][c] = tx.x; in.xp[u][1][c] = tx.y;
+                    } else {
+                        in.xp[u][0][c] = Xs[(size_t)c * n + 2 * p]; in.xp[u][1][c] = Xs[(size_t)c * n + 2 * p + 1];
+                    }
+                }
+            } else if (p < pend) {
+                in.base[u][0] = lws[2 * p]; in.base[u][1] = 0.0;
+#pragma unroll
+                for (int c = 0; c < D; c++) { in.xp[u][0][c] = Xs[(size_t)c * n + 2 * p]; in.xp[u][1][c] = 0.0; }
+            }
+        }
+    };
+    auto compute_general = [&](const StepIo &io, int i, const In &in, Acc<D> &ac, Lse3 &ax, double (&l)[2 * kU],
+                               double (&x)[2 * kU][D]) {
+        double av[APF ? 2 * kU : 1];
+        const int64_t qbase = pstart + (int64_t)i * kIt;
+#pragma unroll
+        for (int u = 0; u < kU; u++) {
+            const int64_t p = qbase + u * 32 + lane;
+            if (p < pend) {
+                do_pair<M, FK>(model, a, io, n, vec_x, p, in.xp[u], in.base[u],
+                               reinterpret_cast<double (&)[2][D]>(x[2 * u]), l + 2 * u, APF ? av + 2 * u : av);
+            } else {
+                l[2 * u] = l[2 * u + 1] = -CUDART_INF;
+                if (APF) av[APF ? 2 * u : 0] = av[APF ? 2 * u + 1 : 0] = -CUDART_INF;
+#pragma unroll
+                for (int c = 0; c < D; c++) { x[2 * u][c] = 0.0; x[2 * u + 1][c] = 0.0; }
+            }
+        }
+        acc_add_batch<2 * kU, D>(ac, l, x, mom);
+        if (APF) lse3_add_batch<(APF ? 2 * kU : 1)>(ax, av);
+    };
+    // dynamic slabs: a warp takes the next slab of `slab_it` consecutive iterations from a shared counter, so
+    // the warps of the SM drift apart (one warp's loads overlap the others' arithmetic) and all retire within
+    // one slab of each other whatever the scheduler's priorities.  Determinism: a slab's statistics are parked in
+    // shared memory as one record per slab -- the 32 lanes' own (max, sum exp, sum exp^2), or, when auxiliary
+    // weights / moments make that too large, their fixed-order reduction over the warp -- and write_partial
+    // merges the records in slab order, so the result does not depend on which warp ran which slab.  The tail of
+    // the range is cut into single-iteration slabs (short drain).  The records alias the CDF staging buffers,
+    // which only the resampling branch uses.
+    const int slab_it = a.slab_it;
+    const int n_small = a.slab_small < n_iter ? a.slab_small : n_iter;
+    const int it_small0 = n_iter - n_small;                               // first single-iteration slab
+    const int n_big = (it_small0 + slab_it - 1) / slab_it;                // slabs of (up to) slab_it iterations
+    const int n_slab = n_big + n_small;
+    const bool lane_rec = a.slab_lane != 0;
+    auto grab = [&]() {
+        int v = 0;
+        if (lane == 0) v = atomicAdd(&sh.next, 1);
+        return __shfl_sync(0xffffffffu, v, 0);
+    };
+    auto first_it = [&](int sl) { return sl < n_big ? sl * slab_it : it_small0 + (sl - n_big); };
+    auto park = [&](double *rec, const Acc<D> &sa, const Lse3 &sx) {
+        if (lane_rec) { rec[lane] = sa.w.m; rec[32 + lane] = sa.w.s; rec[64 + lane] = sa.w.q; }
+        else warp_reduce_to_slab<D, APF>(sa, sx, mom, rec, lane);
+    };
+    // software pipeline (1-D states): the inputs of the next iteration -- of this slab, or of the slab the warp
+    // takes next -- are requested before the current iteration's arithmetic starts (77.5 vs 80.8 us at 512
+    // threads; at 768 threads / 80 registers it spills: 120 us)
+    constexpr bool PREF = (D == 1);
+    // FUSED: every iteration runs step t and then step t + 1 on the values step t has just stored -- exactly what
+    // the unfused step t + 1 would load -- with the same slabs, lanes and batches, so both steps' records and
+    // partial rows carry the bits of two separate launches.  Step t + 1's records go to the CTA's slice of
+    // fuse_slab (the shared-memory buffer holds step t's).  In place: step t + 1 writes buffers [(t+1) & 1] =
+    // [(t-1) & 1], the pass's input.  Every element is read once, by the thread that later overwrites it, and its
+    // store depends on that load, so no thread ever reads a value another thread wrote; these loads therefore go
+    // through plain pointers (no __restrict__, no non-coherent loads).
+    // (no prefetch in a fused pair: its two steps of arithmetic per load cover the load latency, and the
+    // registers of a prefetched iteration would spill)
+    constexpr bool PF = PREF && !FUSED;
+    const StepIo io1 = FUSED ? step_io(a, io0.t + 1, NZ) : io0;
+    const double *Xs = FUSED ? a.X[e.cur] : Xi;
+    const double *lws = FUSED ? a.lw[e.cur] : lwi;
+    const double *Xs_c = FUSED ? Xs + 2 * pstart : Xi_c;
+    const double *lws_c = FUSED ? lws + 2 * pstart : lwi_c;
+    double *const slab1 = FUSED ? a.fuse_slab + (size_t)blockIdx.x * StepCfg<M>::kSlabDoubles : nullptr;
+    int sl = grab();
+    In pre;
+    bool have = false;
+    if (PF && sl < n_slab && fast_ok && first_it(sl) < n_full) {
+        load_full(Xs_c, lws_c, first_it(sl), pre);
+        have = true;
+    }
+    while (sl < n_slab) {
+        const int i0 = first_it(sl);
+        const int rem = it_small0 - i0;
+        const int cnt = sl < n_big ? (rem < slab_it ? rem : slab_it) : 1;
+        Acc<D> sa, sb;
+        acc_init(sa);
+        Lse3 sx = lse3_empty(), sy = lse3_empty();
+        if (FUSED) acc_init(sb);
+        int nsl = n_slab;
+        for (int k_ = 0; k_ < cnt; k_++) {
+            const int i = i0 + k_;
+            In cin;
+            const bool cur_have = have;
+            if (PF && have) cin = pre;
+            int inext = -1;
+            if (k_ + 1 < cnt) inext = i + 1;
+            else { nsl = grab(); if (nsl < n_slab) inext = first_it(nsl); }
+            have = false;
+            if (PF && inext >= 0 && fast_ok && inext < n_full) { load_full(Xs_c, lws_c, inext, pre); have = true; }
+            const bool full = fast_ok && i < n_full;
+            if (!(PF && cur_have)) {
+                if (full) load_full(Xs_c, lws_c, i, cin);
+                else load_general(Xs, lws, i, cin);
+            }
+            double l[2 * kU], x[2 * kU][D];
+            if (full) compute_full(io0, i, cin, sa, sx, l, x);
+            else compute_general(io0, i, cin, sa, sx, l, x);
+            if (FUSED) {
+                In nx;
+#pragma unroll
+                for (int u = 0; u < kU; u++) {
+#pragma unroll
+                    for (int j2 = 0; j2 < 2; j2++) {
+                        nx.base[u][j2] = l[2 * u + j2];
+#pragma unroll
+                        for (int c = 0; c < D; c++) nx.xp[u][j2][c] = x[2 * u + j2][c];
+                    }
+                    // the odd last particle: load_general's (unused) base of the missing partner
+                    if (!full && 2 * (pstart + (int64_t)i * kIt + u * 32 + lane) + 1 == n) nx.base[u][1] = 0.0;
+                }
+                if (full) compute_full(io1, i, nx, sb, sy, l, x);
+                else compute_general(io1, i, nx, sb, sy, l, x);
+            }
+        }
+        park(s_stage + (size_t)sl * a.slab_stride, sa, sx);
+        if (FUSED) park(slab1 + (size_t)sl * a.slab_stride, sb, sy);
+        sl = nsl;
+    }
+    return n_slab;
+}
+
+// A step the prologue says does not resample: the streaming pass (D = 1 and `fuse`: a fused pair).  A speculating
+// shard then collects the peers' statistics (`dec`); if the global test says "resample" after all, the pass is
+// discarded and this returns true.
+template <class M, int FK>
+__device__ __forceinline__ bool stream_step(const M &model, const FilterArgs &a, const StepEnv &e, bool fuse,
+                                            bool speculate, PrologueCarry &pc, StepDecision &dec, StepSmem &sh,
+                                            double *s_stage, int &n_slab) {
+    if constexpr (M::D == 1) {
+        n_slab = fuse ? stream_pass<M, FK, true>(model, a, e, sh, s_stage) : stream_pass<M, FK, false>(model, a, e, sh, s_stage);
+    } else {
+        n_slab = stream_pass<M, FK, false>(model, a, e, sh, s_stage);
+    }
+    if (!speculate) return false;
+    // now the peers' statistics: bookkeeping, and was the guess right?
+    __syncthreads();
+    dec = prologue_end<FkTraits<FK>::apf, StepCfg<M>::BS>(a, e.io.t, sh, blockIdx.x == 0, true, pc);
+    if (!dec.rs) return false;
+    // no: discard the pass, take the resampling branch
+    n_slab = 0;
+    if (threadIdx.x == 0) sh.next = 0;
+    __syncthreads();
+    return true;
+}
+
+// The first half of a resampling step, A = resampling(scheme, aux.W, M=N) (core.py:329-333): the CDF of this CTA's
+// range -- with the ancestor hints scattered to A when a counting scheme resamples locally -- the multinomial
+// spacings, and the grid barrier after which every CTA may read the whole CDF.
+template <class M, int FK, int SCHEME>
+__device__ __forceinline__ void resample_scan(const M &model, const FilterArgs &a, const StepEnv &e,
+                                              const StepDecision &dec, double u_sys, StepSmem &sh, double *s_stage,
+                                              double *s_warp) {
+    constexpr int BS = StepCfg<M>::BS, kStage = StepCfg<M>::kStage;
+    constexpr int kBarriers = (SCHEME == SMCB_RS_MULTINOMIAL) ? 2 : 1;     // grid barriers per resampling step
+    const int64_t n = e.n, pstart = e.pstart, pend = e.pend;
+    unsigned long long bar_target = (unsigned long long)gridDim.x * ((unsigned long long)dec.nrs_prev * kBarriers);
+    constexpr bool kCount = (SCHEME != SMCB_RS_MULTINOMIAL);      // offspring counting (local resampling only)
+    const bool count_path = kCount && !a.rs_global;
+    {
+        LoadWeights<M, FK> load;
+        load.lw = a.lw[e.cur];
+        load.X = a.X[e.cur];
+        load.ntot = n;
+        load.m = dec.xm;
+        load.s = dec.xs;
+        load.model = model;
+        load.kprev = e.kprev;
+        const int64_t e1 = 2 * pend < n ? 2 * pend : n;
+        if (count_path) {
+            Scatter sc{a.A, (double)n, (SCHEME == SMCB_RS_SYSTEMATIC) ? u_sys : 0.0, (long long)n};
+            if (threadIdx.x == 0) sh.timeout_ptr = a.sync_timeout;
+            scan_scatter_groups<BS, kScanGroupWarps>(load, 2 * pstart, e1, dec.p_b, dec.p_next, a.cdf, sc,
+                                                     blockIdx.x == gridDim.x - 1, sh, reinterpret_cast<int *>(s_stage),
+                                                     4 * kStage);
+        } else {
+            scan_range<BS>(load, 2 * pstart, e1, dec.p_b, dec.p_next, a.cdf, s_warp);
+        }
+    }
+    if (SCHEME == SMCB_RS_MULTINOMIAL) {
+        spacings_pass1<BS>(a, e.io.t, sh);
+        bar_target += gridDim.x;
+        grid_barrier(a, bar_target);
+        spacings_pass2<BS>(a, sh, s_warp);
+    }
+    bar_target += gridDim.x;
+    grid_barrier(a, bar_target);
+}
+
+// the shared tail of the move passes: gather the ancestors' states (Xp = X[A]), restart the weights (reset_weights),
+// write A, propagate and reweight pair p
+template <class M, int FK>
+__device__ __forceinline__ void finish_pair(const M &model, const FilterArgs &a, const StepEnv &e, double reset_c,
+                                            Acc<M::D> &acc, Lse3 &aux, int64_t p, const double *X0, const double *X1,
+                                            int64_t a0, int64_t a1, long long g0, long long g1, bool write_A = true) {
+    constexpr bool APF = FkTraits<FK>::apf;
+    constexpr int D = M::D, NZ = M::NZ;
+    const int64_t n = e.n;
+    double *__restrict__ Xo = e.io.Xo;
+    double *__restrict__ lwo = e.io.lwo;
+    double xp[2][D], base[2], x[2][D];
+#pragma unroll
+    for (int c = 0; c < D; c++) {                // Xp = X[A], component-wise (SoA)
+        xp[0][c] = __ldg(X0 + (size_t)c * n + a0);
+        xp[1][c] = __ldg(X1 + (size_t)c * n + a1);
+    }
+    if (APF) {   // core.py:302: lw = log_mean_exp(logetat, W) - logetat[A]
+        base[0] = reset_c - model_logeta<M>(model, e.kprev, xp[0]);
+        base[1] = reset_c - model_logeta<M>(model, e.kprev, xp[1]);
+    } else {     // Weights() then add(delta): lw = 0 + delta (shard mass if sharded)
+        base[0] = reset_c; base[1] = reset_c;
+    }
+    if (write_A) {
+        if (2 * p + 1 < n) *reinterpret_cast<longlong2 *>(a.A + 2 * p) = make_longlong2(g0, g1);
+        else a.A[2 * p] = g0;
+    }
+    double l[2], av[2];
+    if (e.io.zin == nullptr && e.vec_x && 2 * p + 1 < n) {       // complete pair, device normals: no bounds tests
+        double z[2][NZ];
+        tab_normals<NZ>(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)e.io.t, z);
+        const bool odd = move_pair<M, FK, false>(model, e.io.k, xp, base, z, APF && e.io.last_apf, x, l, av);
+#pragma unroll
+        for (int c = 0; c < D; c++) st2(Xo + (size_t)c * n + 2 * p, x[0][c], x[1][c]);
+        st2(lwo + 2 * p, l[0], l[1]);
+        if (!odd) acc_add_batch<2, D, true>(acc, l, x, e.mom);
+        else acc_add_batch<2, D, false>(acc, l, x, e.mom);
+    } else {
+        do_pair<M, FK>(model, a, e.io, n, e.vec_x, p, xp, base, x, l, av);
+        acc_add_batch<2, D>(acc, l, x, e.mom);
+    }
+    if (APF) lse3_add_batch<2>(aux, av);
+}
+
+// the exact answer of np.searchsorted(cdf, su, 'left') from any starting point a0: gallop to a bracket, then bisect
+// (O(log distance) loads)
+__device__ __forceinline__ long long settle(const double *cdf, int64_t n, long long a0, double su) {
+    a0 = a0 < 0 ? 0 : (a0 > n - 1 ? n - 1 : a0);
+    long long lo_, hi_;                                  // answer in [lo_, hi_]: cdf[lo_-1] < su, cdf[hi_] >= su or hi_ = n-1
+    if (__ldcg(cdf + a0) < su) {                         // go up
+        long long step = 1;
+        lo_ = a0 + 1;
+        hi_ = a0 + 1;
+        while (hi_ < n - 1 && __ldcg(cdf + hi_) < su) { lo_ = hi_ + 1; hi_ += step; step <<= 1; }
+        if (hi_ > n - 1) hi_ = n - 1;
+    } else {                                             // go down
+        long long step = 1;
+        hi_ = a0;
+        lo_ = a0 - 1;
+        while (lo_ >= 0 && __ldcg(cdf + lo_) >= su) { hi_ = lo_; lo_ -= step; step <<= 1; }
+        lo_ = lo_ < 0 ? 0 : lo_ + 1;
+    }
+    while (lo_ < hi_) {                                  // first j in [lo_, hi_] with cdf[j] >= su
+        const long long mid = lo_ + ((hi_ - lo_) >> 1);
+        if (__ldcg(cdf + mid) < su) lo_ = mid + 1; else hi_ = mid;
+    }
+    return lo_;
+}
+
+// Move pass of the counting schemes (local resampling): every output verifies the scattered ancestor against the
+// exact su_k (cdf[a-1] < su_k <= cdf[a], i.e. np.searchsorted's answer), walks if the hint is off, then gathers,
+// propagates and reweights.  No tiles, no block barriers: a pair per thread, strided over the CTA's range.
+template <class M, int FK, int SCHEME>
+__device__ __forceinline__ void move_counted(const M &model, const FilterArgs &a, const StepEnv &e, double reset_c,
+                                             double u_sys, const double *uin, Acc<M::D> &acc, Lse3 &aux) {
+    constexpr int BS = StepCfg<M>::BS;
+    const long long t = e.io.t;
+    const int64_t n = e.n, pstart = e.pstart, pend = e.pend;
+    const double *__restrict__ Xi = a.X[e.cur];
+    const double M_ = (double)n;
+    constexpr int kR = kMovePairs;                          // pairs in flight per thread
+    // one round = kR pairs per thread, in three parts: the hints (A, written by the scan), the CDF entries that
+    // verify them, and verify + repair + gather + propagate
+    struct Hints { long long h[kR][2]; };
+    struct Cdf { double c0[kR][2], cm[kR][2], c1[kR][(SCHEME == SMCB_RS_STRATIFIED) ? 2 : 1]; };
+    auto ld_hints = [&](int64_t p0, Hints &H) {
+#pragma unroll
+        for (int r = 0; r < kR; r++) {
+            const int64_t p = p0 + (int64_t)r * BS;
+            H.h[r][0] = H.h[r][1] = 0;
+            if (p < pend && 2 * p + 1 < n) {
+                const longlong2 hh = __ldcg(reinterpret_cast<const longlong2 *>(a.A + 2 * p));
+                H.h[r][0] = hh.x; H.h[r][1] = hh.y;
+            } else if (p < pend) {
+                H.h[r][0] = __ldcg(a.A + 2 * p);
+            }
+        }
+    };
+    auto ld_cdf = [&](int64_t p0, const Hints &H, Cdf &Cc) {
+#pragma unroll
+        for (int r = 0; r < kR; r++) {
+            const int64_t p = p0 + (int64_t)r * BS;
+#pragma unroll
+            for (int q = 0; q < 2; q++) {                    // the two CDF entries that decide the hint
+                long long hh = H.h[r][q];
+                hh = hh < 0 ? 0 : (hh > n - 1 ? n - 1 : hh);
+                const bool on = (p < pend) && (q == 0 || 2 * p + 1 < n);
+                // (plain loads: this SM touches these lines for the first time in this launch, after the grid
+                // barrier, so L1 cannot hold an older copy -- and neighbouring outputs reuse them)
+                Cc.c0[r][q] = on ? a.cdf[hh] : 2.0;
+                Cc.cm[r][q] = (on && hh > 0) ? a.cdf[hh - 1] : -1.0;
+                // stratified: the hint answers k / N and su_k lies up to 1 / N further, so about half of the
+                // outputs belong to the NEXT entry -- fetch it with the other two instead of walking
+                if (SCHEME == SMCB_RS_STRATIFIED) Cc.c1[r][q] = (on && hh + 1 < n) ? a.cdf[hh + 1] : 2.0;
+            }
+        }
+    };
+    auto process = [&](int64_t p0, const Hints &H, const Cdf &Cc) {
+        long long h[kR][2];
+        double su[kR][2];
+        bool valid[kR], two[kR], moved[kR];
+#pragma unroll
+        for (int r = 0; r < kR; r++) {
+            const int64_t p = p0 + (int64_t)r * BS;
+            moved[r] = false;
+            valid[r] = p < pend;
+            two[r] = valid[r] && (2 * p + 1 < n);
+            grid_pair<SCHEME>(u_sys, a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t, uin, p, valid[r],
+                              two[r], M_, su[r][0], su[r][1]);
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                long long hh = H.h[r][q];
+                hh = hh < 0 ? 0 : (hh > n - 1 ? n - 1 : hh);
+                moved[r] = moved[r] || hh != H.h[r][q];
+                h[r][q] = hh;
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < kR; r++) {
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                const bool on = q == 0 ? valid[r] : two[r];
+                bool ok = (Cc.cm[r][q] < su[r][q]) && (su[r][q] <= Cc.c0[r][q] || h[r][q] == n - 1);
+                if (SCHEME == SMCB_RS_STRATIFIED) {
+                    if (on && !ok && Cc.c0[r][q] < su[r][q] && (su[r][q] <= Cc.c1[r][q] || h[r][q] + 1 == n - 1)) {
+                        h[r][q] += 1; moved[r] = true; ok = true;
+                    }
+                }
+                if (on && !ok && Cc.c0[r][q] < su[r][q] && h[r][q] + 1 < n) {
+                    // the hint is too low: ONE round trip for the next kWin entries (independent loads, mostly
+                    // one line) instead of a chain of dependent ones; the search below only runs past them
+                    constexpr int kWin = 6;
+                    const long long b = h[r][q] + 1;
+                    double wv[kWin];
+#pragma unroll
+                    for (int i = 0; i < kWin; i++) wv[i] = (b + i < n) ? __ldcg(a.cdf + b + i) : 2.0;
+                    int cnt = 0;
+#pragma unroll
+                    for (int i = 0; i < kWin; i++) cnt += (wv[i] < su[r][q]) ? 1 : 0;   // monotone CDF: a prefix
+                    if (cnt < kWin) {
+                        long long hn = b + cnt;
+                        h[r][q] = hn > n - 1 ? n - 1 : hn;
+                        moved[r] = true; ok = true;
+                    }
+                }
+                if (on && !ok) {
+                    h[r][q] = settle(a.cdf, n, h[r][q], su[r][q]);
+                    moved[r] = true;
+                }
+            }
+            if (!two[r]) h[r][1] = h[r][0];
+        }
+#pragma unroll
+        for (int r = 0; r < kR; r++) {
+            const int64_t p = p0 + (int64_t)r * BS;
+            if (valid[r]) finish_pair<M, FK>(model, a, e, reset_c, acc, aux, p, Xi, Xi, h[r][0], h[r][1], h[r][0], h[r][1],
+                                             moved[r]);
+        }
+    };
+    constexpr int64_t kStep = (int64_t)kR * BS;
+    for (int64_t p0 = pstart + threadIdx.x; p0 < pend; p0 += kStep) {
+        Hints H;
+        Cdf Cc;
+        ld_hints(p0, H);
+        ld_cdf(p0, H, Cc);
+        process(p0, H, Cc);
+    }
+}
+
+// Move pass of the multinomial scheme (local resampling; every other scheme counts offspring when it resamples
+// locally): per tile of 2 BS outputs, the CDF slice their ancestors lie in is staged in shared memory by one TMA bulk
+// copy (double-buffered) and searched there.
+template <class M, int FK>
+__device__ __forceinline__ void move_tiles(const M &model, const FilterArgs &a, const StepEnv &e, double reset_c,
+                                           Acc<M::D> &acc, Lse3 &aux, double *s_stage, double *s_su, uint64_t *s_bar,
+                                           long long &s_hi) {
+    constexpr int BS = StepCfg<M>::BS, kStage = StepCfg<M>::kStage;
+    const int64_t n = e.n, pstart = e.pstart, pend = e.pend;
+    const double *__restrict__ Xi = a.X[e.cur];
+    const double zlast = __ldcg(a.su + n);
+    int64_t lo = -1;
+    if (threadIdx.x == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_init_fence(); }
+    __syncthreads();
+    uint32_t phase0 = 0, phase1 = 0;
+    int buf = 0;
+    // thread 0: bring cdf[sb, sb + c) into buffer b (sb = lo_ rounded down to even => 16-byte aligned)
+    // by ONE TMA bulk copy (cp.async.bulk + mbarrier); the slice of tile i+1 is in flight while tile i
+    // propagates and reweights
+    auto issue = [&](int64_t lo_, int b) {
+        const int64_t sb = lo_ & ~(int64_t)1;
+        const int c = (int)((n - sb) < kStage ? (n - sb) : kStage);
+        const uint32_t bytes = (uint32_t)(c & ~1) * 8u;
+        double *dst = s_stage + (size_t)b * kStage;
+        if (c & 1) dst[c - 1] = __ldcg(a.cdf + sb + c - 1);      // odd tail (n odd, end of the array)
+        if (bytes) {
+            mbar_arrive_expect_tx(&s_bar[b], bytes);
+            tma_bulk_g2s(dst, a.cdf + sb, bytes, &s_bar[b]);
+        } else {
+            mbar_arrive(&s_bar[b]);
+        }
+    };
+    for (int64_t pbase = pstart; pbase < pend; pbase += BS) {
+        const int64_t p = pbase + threadIdx.x;
+        const bool active = p < pend;
+        const int64_t k0 = 2 * pbase;                                       // first / last output of the tile
+        const int64_t ptop = pbase + BS < pend ? pbase + BS : pend;
+        const int64_t k1 = (2 * ptop < n ? 2 * ptop : n) - 1;
+        double su[2] = {2.0, 2.0};
+        if (active) {
+            su[0] = __ldcg(a.su + 2 * p) / zlast;                   // resampling.py:537
+            su[1] = (2 * p + 1 < n) ? __ldcg(a.su + 2 * p + 1) / zlast : 2.0;
+            if (2 * p == k0) s_su[0] = su[0];
+            if (2 * p == k1) s_su[1] = su[0];
+            if (2 * p + 1 == k1) s_su[1] = su[1];
+        }
+        __syncthreads();
+        const double su_first = s_su[0], su_last = s_su[1];
+        if (lo < 0) {                                      // first tile of this block
+            lo = block_lower_bound<BS>(a.cdf, 0, n, su_first);
+            lo = lo < n - 1 ? lo : n - 1;
+            if (threadIdx.x == 0) issue(lo, buf);
+            __syncthreads();
+        }
+        // su is sorted, so the slice starts at `lo`
+        const int64_t sbase = lo & ~(int64_t)1;
+        const int cnt = (int)((n - sbase) < kStage ? (n - sbase) : kStage);
+        mbar_wait(&s_bar[buf], buf ? phase1 : phase0);
+        if (buf) phase1 ^= 1u; else phase0 ^= 1u;
+        const double *s_cdf = s_stage + (size_t)buf * kStage;
+        const bool covered = (sbase + cnt >= n) || (s_cdf[cnt - 1] >= su_last);
+        int64_t hi = lo;
+        if (!covered) hi = block_lower_bound<BS>(a.cdf, lo, n, su_last);   // rare: sparse mass
+        int64_t a0 = 0, a1 = 0;
+        if (active) {
+            if (covered) {
+                int l0, l1;
+                tile_search(s_cdf, (int)(lo - sbase), cnt, su[0], su[1], l0, l1);
+                a0 = sbase + l0;
+                a1 = sbase + l1;
+                if (2 * p == k1) s_hi = a0;
+                if (2 * p + 1 == k1) s_hi = a1;
+            } else {
+                const int64_t hi1 = hi < n ? hi + 1 : n;
+                a0 = lower_bound_cg(a.cdf, lo, hi1, su[0]);
+                a1 = lower_bound_cg(a.cdf, a0, hi1, su[1]);
+            }
+        }
+        __syncthreads();                                   // s_hi published; buffer buf^1 is free
+        const int64_t lo_next = covered ? (s_hi < n ? s_hi : n - 1) : (hi < n ? hi : n - 1);
+        if (pbase + BS < pend && threadIdx.x == 0) issue(lo_next, buf ^ 1);
+        if (active) {
+            a0 = a0 < n - 1 ? a0 : n - 1;
+            a1 = a1 < n - 1 ? a1 : n - 1;
+            finish_pair<M, FK>(model, a, e, reset_c, acc, aux, p, Xi, Xi, a0, a1, a0, a1);
+        }
+        lo = lo_next;
+        buf ^= 1;
+    }
+}
+
+// Move pass of the exact global resampling over particle shards (SURVEY.md section 8e, mode 2; resampling.py:599-610
+// applied to the concatenation of all shards).  Output j of rank r is global offspring index_offset + j: its grid
+// point su is located in the global CDF in two levels -- shard k with goff[k] <= su < goff[k+1] (offsets from the
+// exchanged statistics, identical bits on every rank), then v = (su - goff[k]) / gpi[k] in shard k's own normalised
+// CDF, read over NVLink -- and the ancestor's state is pulled from shard k's particle buffer.
+template <class M, int FK, int SCHEME>
+__device__ __forceinline__ void move_global(const M &model, const FilterArgs &a, const StepEnv &e, double reset_c,
+                                            double u_sys, const double *uin, Acc<M::D> &acc, Lse3 &aux, StepSmem &sh,
+                                            double *s_stage, double *s_su, long long &s_hi) {
+    constexpr int BS = StepCfg<M>::BS, kStage = StepCfg<M>::kStage;
+    const long long t = e.io.t;
+    const int cur = e.cur;
+    const int64_t n = e.n, pstart = e.pstart, pend = e.pend;
+    // First: tell every peer that this shard's CDF of step t is complete, and wait for theirs.
+    if (blockIdx.x == 0 && (int)threadIdx.x < a.world) {
+        __threadfence_system();
+        double *slot = a.mail_peer[threadIdx.x] + ((size_t)(t & 1) * a.world + a.rank) * kMailStride;
+        *reinterpret_cast<volatile double *>(slot + kMailScan) = (double)(t + 1);
+    }
+    if ((int)threadIdx.x < a.world)
+        wait_epoch(a.mail_local + ((size_t)(t & 1) * a.world + threadIdx.x) * kMailStride + kMailScan,
+                   (double)(t + 1), a.sync_timeout);
+    __syncthreads();
+    const int world = a.world;
+    const double M_ = (double)a.n_global;
+    double *s_cdf = s_stage;
+    int64_t lo = -1;
+    int lo_shard = -1;
+    for (int64_t pbase = pstart; pbase < pend; pbase += BS) {
+        const int64_t p = pbase + threadIdx.x;
+        const bool active = p < pend;                               // sharded filters have even n
+        const int64_t k0 = 2 * pbase;
+        const int64_t ptop = pbase + BS < pend ? pbase + BS : pend;
+        const int64_t k1 = 2 * ptop - 1;
+        double su[2] = {2.0, 2.0};
+        if (active) {
+            const double g0 = (double)(a.index_offset + 2 * p);
+            if (SCHEME == SMCB_RS_SYSTEMATIC) {
+                su[0] = (u_sys + g0) / M_;
+                su[1] = (u_sys + (g0 + 1.0)) / M_;
+            } else {
+                double u0, u1;
+                if (uin) { u0 = uin[2 * p]; u1 = uin[2 * p + 1]; }
+                else uniform_pair(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t, kPurposeUniform, u0, u1);
+                su[0] = (u0 + g0) / M_;
+                su[1] = (u1 + (g0 + 1.0)) / M_;
+            }
+            if (2 * p == k0) s_su[0] = su[0];
+            if (2 * p + 1 == k1) s_su[1] = su[1];
+        }
+        __syncthreads();
+        const double su_first = s_su[0], su_last = s_su[1];
+        const int kf = shard_of(sh.goff, sh.gpi, world, su_first);
+        const int kl = shard_of(sh.goff, sh.gpi, world, su_last);
+        int ks[2] = {kf, kf};
+        int64_t an[2] = {0, 0};
+        if (kf == kl) {
+            // the whole tile draws from one shard: staged search on that shard's CDF with the grid
+            // points mapped into its local scale
+            const double *cdf = a.pcdf[kf];
+            const double off = sh.goff[kf], pi = sh.gpi[kf];
+            const double v0 = fmin((su[0] - off) / pi, 1.0), v1 = fmin((su[1] - off) / pi, 1.0);
+            const double v_first = fmin((su_first - off) / pi, 1.0), v_last = fmin((su_last - off) / pi, 1.0);
+            if (lo < 0 || lo_shard != kf) lo = block_lower_bound<BS>(cdf, 0, n, v_first);
+            if (lo > n - 1) lo = n - 1;
+            lo_shard = kf;
+            const int64_t sbase = lo & ~(int64_t)1;
+            const int cnt = (int)((n - sbase) < kStage ? (n - sbase) : kStage);
+            for (int i = 2 * threadIdx.x; i < cnt; i += 2 * BS) {
+                if (i + 1 < cnt) *reinterpret_cast<double2 *>(&s_cdf[i]) = __ldcg(reinterpret_cast<const double2 *>(cdf + sbase + i));
+                else s_cdf[i] = __ldcg(cdf + sbase + i);
+            }
+            __syncthreads();
+            const bool covered = (sbase + cnt >= n) || (s_cdf[cnt - 1] >= v_last);
+            int64_t hi = lo;
+            if (!covered) hi = block_lower_bound<BS>(cdf, lo, n, v_last);
+            if (active) {
+                if (covered) {
+                    int l0, l1;
+                    tile_search(s_cdf, (int)(lo - sbase), cnt, v0, v1, l0, l1);
+                    an[0] = sbase + l0;
+                    an[1] = sbase + l1;
+                    if (2 * p + 1 == k1) s_hi = an[1];
+                } else {
+                    const int64_t hi1 = hi < n ? hi + 1 : n;
+                    an[0] = lower_bound_cg(cdf, lo, hi1, v0);
+                    an[1] = lower_bound_cg(cdf, an[0], hi1, v1);
+                }
+            }
+            __syncthreads();
+            lo = covered ? (s_hi < n ? s_hi : n - 1) : (hi < n ? hi : n - 1);
+        } else {
+            // the tile straddles a shard boundary (at most world - 1 tiles per rank): plain searches
+            if (active) {
+#pragma unroll
+                for (int j = 0; j < 2; j++) {
+                    ks[j] = shard_of(sh.goff, sh.gpi, world, su[j]);
+                    const double v = fmin((su[j] - sh.goff[ks[j]]) / sh.gpi[ks[j]], 1.0);
+                    an[j] = lower_bound_cg(a.pcdf[ks[j]], 0, n, v);
+                }
+            }
+            lo = -1;
+        }
+        if (active) {
+            const int64_t a0 = an[0] < n - 1 ? an[0] : n - 1, a1 = an[1] < n - 1 ? an[1] : n - 1;
+            // ancestors are GLOBAL particle indices
+            finish_pair<M, FK>(model, a, e, reset_c, acc, aux, p, a.pX[ks[0]][cur], a.pX[ks[1]][cur], a0, a1,
+                               (long long)ks[0] * n + a0, (long long)ks[1] * n + a1);
+        }
+        __syncthreads();       // s_su / s_hi / s_cdf are rewritten by the next tile
+    }
+}
+
 // ---------------------------------------------------------------------------
 // the step kernel: resample_move + reweight_particles (+ compute_summaries of the previous step)
 // (core.py:323-367)
@@ -1211,7 +1932,6 @@ template <class M, int FK, int SCHEME>
 __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs a, long long t) {
     constexpr bool APF = FkTraits<FK>::apf;
     constexpr int D = M::D, NZ = M::NZ, BS = StepCfg<M>::BS;
-    constexpr int kStage = StepCfg<M>::kStage;
     extern __shared__ __align__(128) double s_dyn[];    // math tables | [2][kStage] CDF slices (resampling branch)
     double *const s_stage = s_dyn + kMathTabDoubles;
     __shared__ StepSmem sh;
@@ -1262,694 +1982,36 @@ __global__ void __launch_bounds__(StepCfg<M>::BS, 1) k_step(M model, FilterArgs 
         fuse = a.fuse_mode == 2 || 2.0 * dec.ess - ess2 >= (double)a.n_global * a.essrmin;
     }
     if (fuse && blockIdx.x == 0 && threadIdx.x == 0) { a.fuse[0] = t + 1; a.fuse[1] += 1; }
-    double reset_c = dec.reset_c;
-    const StepIo io0 = step_io(a, t, NZ);
-    const StepK &k = io0.k;
-    const StepK kprev = step_consts(a, t - 1);
-    const double *__restrict__ Xi = a.X[cur];
-    const double *__restrict__ lwi = a.lw[cur];
-    double *__restrict__ Xo = io0.Xo;
-    double *__restrict__ lwo = io0.lwo;
-    const int64_t n = a.n;
-    const double *zin = io0.zin;
-    const bool last_apf = APF && io0.last_apf;
-    const bool mom = a.moments != nullptr;
-    const bool vec_x = (D == 1) || ((n & 1) == 0);     // SoA component rows are 16-byte aligned
-    int64_t pstart, pend;
-    cta_range(a, pstart, pend);
+    StepEnv e;
+    e.io = step_io(a, t, NZ);
+    e.kprev = step_consts(a, t - 1);
+    e.cur = cur;
+    e.n = a.n;
+    e.vec_x = (D == 1) || ((a.n & 1) == 0);
+    e.mom = a.moments != nullptr;
+    cta_range(a, e.pstart, e.pend);
 
     Acc<D> acc;
     acc_init(acc);
     Lse3 aux = lse3_empty();
-    int n_slab = 0;                                    // slab records of the streaming branch
-
-    // propagate + reweight one pair of particles by step io.t; writes x', lw'; returns x', lw' (and the auxiliary
-    // log-weights of the next step for an APF), -inf in masked slots
-    auto do_pair = [&](const StepIo &io, int64_t p, const double (&xp)[2][D], const double (&base)[2],
-                       double (&x)[2][D], double *l, double *av) {
-        double z[2][NZ];
-        pair_normals<NZ>(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)io.t, io.zin, n, p, z);
-        move_pair<M, FK, false>(model, io.k, xp, base, z, io.last_apf, x, l, av);
-        store_pair<D, APF>(io.Xo, io.lwo, n, p, vec_x, x, l, av);
-    };
-
-    if (!rs) {
-        // A = arange(N), Xp = X (core.py:335-336): pure streaming pass.  Work unit = one "iteration" of a warp:
-        // kU x 32 consecutive pairs (kU coalesced 512-byte rows per array), kU pairs in flight per thread.
-        constexpr int kU = StepCfg<M>::kU;
-        constexpr int kIt = 32 * kU;                                          // pairs per iteration
-        const int lane = threadIdx.x & 31;
-        const int npl = (int)(pend - pstart);                                 // pairs of this CTA (< 2^31)
-        const int n_iter = (npl + kIt - 1) / kIt;
-        // iterations made of complete pairs only run without any bounds test (the odd last particle and the ragged
-        // end of the range take the general path)
-        const int64_t whole = (n >> 1) < pend ? (n >> 1) : pend;
-        const int n_full = whole > pstart ? (int)((whole - pstart) / kIt) : 0;
-        const bool fast_ok = (zin == nullptr) && vec_x;
-        const double *__restrict__ lwi_c = lwi + 2 * pstart;
-        const double *__restrict__ Xi_c = Xi + 2 * pstart;
-        const uint64_t gpair0 = (uint64_t)((a.index_offset >> 1) + pstart);
-        // one iteration: pairs (relative to pstart) i * kIt + u * 32 + lane.  Loads and arithmetic are separate so
-        // that the inputs of the NEXT iteration can be requested before the current one is computed.
-        struct In { double base[kU][2]; double xp[kU][2][D]; };
-        auto load_full = [&](const double *Xs_c, const double *lws_c, int i, In &in) {
-#pragma unroll
-            for (int u = 0; u < kU; u++) {
-                const int o2 = 2 * (i * kIt + u * 32 + lane);
-                const double2 tl = ld2(lws_c + o2);
-                in.base[u][0] = tl.x; in.base[u][1] = tl.y;
-#pragma unroll
-                for (int c = 0; c < D; c++) {
-                    const double2 tx = ld2(Xs_c + (size_t)c * n + o2);
-                    in.xp[u][0][c] = tx.x; in.xp[u][1][c] = tx.y;
-                }
-            }
-        };
-        auto compute_full = [&](const StepIo &io, int i, const In &in, Acc<D> &ac, Lse3 &ax, double (&l)[2 * kU],
-                                double (&x)[2 * kU][D]) {
-            double av[APF ? 2 * kU : 1];
-            bool odd = false;                                 // some value is +-inf / NaN (integer test)
-#pragma unroll
-            for (int u = 0; u < kU; u++) {
-                const int prel = i * kIt + u * 32 + lane;
-                double z[2][NZ];
-                tab_normals<NZ>(a.key, gpair0 + (uint64_t)prel, (uint32_t)io.t, z);
-                // (move_pair's arithmetic written out: this is the streaming pass's inner loop, and it takes one NaN
-                // fix-up per iteration instead of one per pair)
-#pragma unroll
-                for (int j2 = 0; j2 < 2; j2++) {
-                    double d;
-                    model_move<M, FK>(model, io.k, in.xp[u][j2], z[j2], x[2 * u + j2], d);
-                    l[2 * u + j2] = in.base[u][j2] + d;                   // Weights.add, resampling.py:241-244
-                    odd |= nonfinite(l[2 * u + j2]);
-                    if (APF) {
-                        av[APF ? 2 * u + j2 : 0] = io.last_apf ? l[2 * u + j2] + model_logeta<M>(model, io.k, x[2 * u + j2])
-                                                               : -CUDART_INF;
-                        odd |= nonfinite(av[APF ? 2 * u + j2 : 0]);
-                    }
-                }
-            }
-            if (odd) {                                        // rare: NaN -> -inf (resampling.py:220)
-#pragma unroll
-                for (int q = 0; q < 2 * kU; q++) {
-                    l[q] = fix_nan(l[q]);
-                    if (APF) av[APF ? q : 0] = fix_nan(av[APF ? q : 0]);
-                }
-            }
-            double *const lwo_c = io.lwo + 2 * pstart;
-            double *const Xo_c = io.Xo + 2 * pstart;
-#pragma unroll
-            for (int u = 0; u < kU; u++) {
-                const int o2 = 2 * (i * kIt + u * 32 + lane);
-#pragma unroll
-                for (int c = 0; c < D; c++) st2(Xo_c + (size_t)c * n + o2, x[2 * u][c], x[2 * u + 1][c]);
-                st2(lwo_c + o2, l[2 * u], l[2 * u + 1]);
-            }
-            if (!odd) {
-                acc_add_batch<2 * kU, D, true>(ac, l, x, mom);
-            } else {
-                acc_add_batch<2 * kU, D, false>(ac, l, x, mom);
-            }
-            if (APF) lse3_add_batch<(APF ? 2 * kU : 1)>(ax, av);
-        };
-        // general path: ragged end of the range, the odd last particle, injected normals, odd SoA stride
-        auto load_general = [&](const double *Xs, const double *lws, int i, In &in) {
-            const int64_t qbase = pstart + (int64_t)i * kIt;
-#pragma unroll
-            for (int u = 0; u < kU; u++) {
-                const int64_t p = qbase + u * 32 + lane;
-                if (p < pend && 2 * p + 1 < n) {
-                    double2 tl = ld2(lws + 2 * p);
-                    in.base[u][0] = tl.x; in.base[u][1] = tl.y;
-#pragma unroll
-                    for (int c = 0; c < D; c++) {
-                        if (vec_x) {
-                            double2 tx = ld2(Xs + (size_t)c * n + 2 * p);
-                            in.xp[u][0][c] = tx.x; in.xp[u][1][c] = tx.y;
-                        } else {
-                            in.xp[u][0][c] = Xs[(size_t)c * n + 2 * p]; in.xp[u][1][c] = Xs[(size_t)c * n + 2 * p + 1];
-                        }
-                    }
-                } else if (p < pend) {
-                    in.base[u][0] = lws[2 * p]; in.base[u][1] = 0.0;
-#pragma unroll
-                    for (int c = 0; c < D; c++) { in.xp[u][0][c] = Xs[(size_t)c * n + 2 * p]; in.xp[u][1][c] = 0.0; }
-                }
-            }
-        };
-        auto compute_general = [&](const StepIo &io, int i, const In &in, Acc<D> &ac, Lse3 &ax, double (&l)[2 * kU],
-                                   double (&x)[2 * kU][D]) {
-            double av[APF ? 2 * kU : 1];
-            const int64_t qbase = pstart + (int64_t)i * kIt;
-#pragma unroll
-            for (int u = 0; u < kU; u++) {
-                const int64_t p = qbase + u * 32 + lane;
-                if (p < pend) {
-                    do_pair(io, p, in.xp[u], in.base[u], reinterpret_cast<double (&)[2][D]>(x[2 * u]), l + 2 * u,
-                            APF ? av + 2 * u : av);
-                } else {
-                    l[2 * u] = l[2 * u + 1] = -CUDART_INF;
-                    if (APF) av[APF ? 2 * u : 0] = av[APF ? 2 * u + 1 : 0] = -CUDART_INF;
-#pragma unroll
-                    for (int c = 0; c < D; c++) { x[2 * u][c] = 0.0; x[2 * u + 1][c] = 0.0; }
-                }
-            }
-            acc_add_batch<2 * kU, D>(ac, l, x, mom);
-            if (APF) lse3_add_batch<(APF ? 2 * kU : 1)>(ax, av);
-        };
-        // dynamic slabs: a warp takes the next slab of `slab_it` consecutive iterations from a shared counter, so
-        // the warps of the SM drift apart (one warp's loads overlap the others' arithmetic) and all retire within
-        // one slab of each other whatever the scheduler's priorities.  Determinism: a slab's statistics are parked in
-        // shared memory as one record per slab -- the 32 lanes' own (max, sum exp, sum exp^2), or, when auxiliary
-        // weights / moments make that too large, their fixed-order reduction over the warp -- and write_partial
-        // merges the records in slab order, so the result does not depend on which warp ran which slab.  The tail of
-        // the range is cut into single-iteration slabs (short drain).  The records alias the CDF staging buffers,
-        // which only the resampling branch uses.
-        const int slab_it = a.slab_it;
-        const int n_small = a.slab_small < n_iter ? a.slab_small : n_iter;
-        const int it_small0 = n_iter - n_small;                               // first single-iteration slab
-        const int n_big = (it_small0 + slab_it - 1) / slab_it;                // slabs of (up to) slab_it iterations
-        n_slab = n_big + n_small;
-        const bool lane_rec = a.slab_lane != 0;
-        auto grab = [&]() {
-            int v = 0;
-            if (lane == 0) v = atomicAdd(&sh.next, 1);
-            return __shfl_sync(0xffffffffu, v, 0);
-        };
-        auto first_it = [&](int sl) { return sl < n_big ? sl * slab_it : it_small0 + (sl - n_big); };
-        auto park = [&](double *rec, const Acc<D> &sa, const Lse3 &sx) {
-            if (lane_rec) { rec[lane] = sa.w.m; rec[32 + lane] = sa.w.s; rec[64 + lane] = sa.w.q; }
-            else warp_reduce_to_slab<D, APF>(sa, sx, mom, rec, lane);
-        };
-        // software pipeline (1-D states): the inputs of the next iteration -- of this slab, or of the slab the warp
-        // takes next -- are requested before the current iteration's arithmetic starts (77.5 vs 80.8 us at 512
-        // threads; at 768 threads / 80 registers it spills: 120 us)
-        constexpr bool PREF = (D == 1);
-        // FUSED: every iteration runs step t and then step t + 1 on the values step t has just stored -- exactly what
-        // the unfused step t + 1 would load -- with the same slabs, lanes and batches, so both steps' records and
-        // partial rows carry the bits of two separate launches.  Step t + 1's records go to the CTA's slice of
-        // fuse_slab (the shared-memory buffer holds step t's).  In place: step t + 1 writes buffers [(t+1) & 1] =
-        // [(t-1) & 1], the pass's input.  Every element is read once, by the thread that later overwrites it, and its
-        // store depends on that load, so no thread ever reads a value another thread wrote; these loads therefore go
-        // through plain pointers (no __restrict__, no non-coherent loads).
-        auto slabs = [&](auto fused) {
-            constexpr bool FUSED = decltype(fused)::value;
-            // (no prefetch in a fused pair: its two steps of arithmetic per load cover the load latency, and the
-            // registers of a prefetched iteration would spill)
-            constexpr bool PF = PREF && !FUSED;
-            const StepIo io1 = FUSED ? step_io(a, t + 1, NZ) : io0;
-            const double *Xs = FUSED ? a.X[cur] : Xi;
-            const double *lws = FUSED ? a.lw[cur] : lwi;
-            const double *Xs_c = FUSED ? Xs + 2 * pstart : Xi_c;
-            const double *lws_c = FUSED ? lws + 2 * pstart : lwi_c;
-            double *const slab1 = FUSED ? a.fuse_slab + (size_t)blockIdx.x * StepCfg<M>::kSlabDoubles : nullptr;
-            int sl = grab();
-            In pre;
-            bool have = false;
-            if (PF && sl < n_slab && fast_ok && first_it(sl) < n_full) {
-                load_full(Xs_c, lws_c, first_it(sl), pre);
-                have = true;
-            }
-            while (sl < n_slab) {
-                const int i0 = first_it(sl);
-                const int rem = it_small0 - i0;
-                const int cnt = sl < n_big ? (rem < slab_it ? rem : slab_it) : 1;
-                Acc<D> sa, sb;
-                acc_init(sa);
-                Lse3 sx = lse3_empty(), sy = lse3_empty();
-                if (FUSED) acc_init(sb);
-                int nsl = n_slab;
-                for (int k_ = 0; k_ < cnt; k_++) {
-                    const int i = i0 + k_;
-                    In cin;
-                    const bool cur_have = have;
-                    if (PF && have) cin = pre;
-                    int inext = -1;
-                    if (k_ + 1 < cnt) inext = i + 1;
-                    else { nsl = grab(); if (nsl < n_slab) inext = first_it(nsl); }
-                    have = false;
-                    if (PF && inext >= 0 && fast_ok && inext < n_full) { load_full(Xs_c, lws_c, inext, pre); have = true; }
-                    const bool full = fast_ok && i < n_full;
-                    if (!(PF && cur_have)) {
-                        if (full) load_full(Xs_c, lws_c, i, cin);
-                        else load_general(Xs, lws, i, cin);
-                    }
-                    double l[2 * kU], x[2 * kU][D];
-                    if (full) compute_full(io0, i, cin, sa, sx, l, x);
-                    else compute_general(io0, i, cin, sa, sx, l, x);
-                    if (FUSED) {
-                        In nx;
-#pragma unroll
-                        for (int u = 0; u < kU; u++) {
-#pragma unroll
-                            for (int j2 = 0; j2 < 2; j2++) {
-                                nx.base[u][j2] = l[2 * u + j2];
-#pragma unroll
-                                for (int c = 0; c < D; c++) nx.xp[u][j2][c] = x[2 * u + j2][c];
-                            }
-                            // the odd last particle: load_general's (unused) base of the missing partner
-                            if (!full && 2 * (pstart + (int64_t)i * kIt + u * 32 + lane) + 1 == n) nx.base[u][1] = 0.0;
-                        }
-                        if (full) compute_full(io1, i, nx, sb, sy, l, x);
-                        else compute_general(io1, i, nx, sb, sy, l, x);
-                    }
-                }
-                park(s_stage + (size_t)sl * a.slab_stride, sa, sx);
-                if (FUSED) park(slab1 + (size_t)sl * a.slab_stride, sb, sy);
-                sl = nsl;
-            }
-        };
-        if constexpr (D == 1) {
-            if (fuse) slabs(std::true_type{});
-            else slabs(std::false_type{});
-        } else {
-            slabs(std::false_type{});
-        }
-        if (!speculate) goto step_done;
-        // now the peers' statistics: bookkeeping, and was the guess right?
-        __syncthreads();
-        dec = prologue_end<APF, BS>(a, t, sh, blockIdx.x == 0, true, pc);
-        if (!dec.rs) goto step_done;
-        // no: discard the pass, take the resampling branch
-        reset_c = dec.reset_c;
-        acc_init(acc);
-        aux = lse3_empty();
-        n_slab = 0;
-        if (threadIdx.x == 0) sh.next = 0;
-        __syncthreads();
-    }
-    {
-        // A = resampling(scheme, aux.W, M=N); Xp = X[A]; reset_weights (core.py:329-333)
-        constexpr int kBarriers = (SCHEME == SMCB_RS_MULTINOMIAL) ? 2 : 1;     // grid barriers per resampling step
-        unsigned long long bar_target = (unsigned long long)gridDim.x * ((unsigned long long)dec.nrs_prev * kBarriers);
-        const double *uin = a.u_in ? a.u_in + (size_t)t * (n + 1) : nullptr;
+    int n_slab = 0;                                    // slab records of the streaming pass
+    // the resampling branch: A = resampling(scheme, aux.W, M=N); Xp = X[A]; reset_weights (core.py:329-333).  (One
+    // short-circuit condition on purpose: a "resample" flag set in both branches and tested after them costs the
+    // bootstrap kernels about 150 more bytes of spills at the 128-register cap.)
+    if (rs || stream_step<M, FK>(model, a, e, fuse, speculate, pc, dec, sh, s_stage, n_slab)) {
+        const double *uin = a.u_in ? a.u_in + (size_t)t * (a.n + 1) : nullptr;
         const double u_sys = (SCHEME == SMCB_RS_SYSTEMATIC) ? systematic_u(a.key, t, uin) : 0.0;
-        constexpr bool kCount = (SCHEME != SMCB_RS_MULTINOMIAL);      // offspring counting (local resampling only)
-        const bool count_path = kCount && !a.rs_global;
-        {
-            LoadWeights<M, FK> load;
-            load.lw = a.lw[cur];
-            load.X = a.X[cur];
-            load.ntot = n;
-            load.m = dec.xm;
-            load.s = dec.xs;
-            load.model = model;
-            load.kprev = kprev;
-            const int64_t e1 = 2 * pend < n ? 2 * pend : n;
-            if (count_path) {
-                Scatter sc{a.A, (double)n, (SCHEME == SMCB_RS_SYSTEMATIC) ? u_sys : 0.0, (long long)n};
-                if (threadIdx.x == 0) sh.timeout_ptr = a.sync_timeout;
-                scan_scatter_groups<BS, kScanGroupWarps>(load, 2 * pstart, e1, dec.p_b, dec.p_next, a.cdf, sc,
-                                                         blockIdx.x == gridDim.x - 1, sh, reinterpret_cast<int *>(s_stage),
-                                                         4 * kStage);
-            } else {
-                scan_range<BS>(load, 2 * pstart, e1, dec.p_b, dec.p_next, a.cdf, s_warp);
-            }
-        }
-        if (SCHEME == SMCB_RS_MULTINOMIAL) {
-            spacings_pass1<BS>(a, t, sh);
-            bar_target += gridDim.x;
-            grid_barrier(a, bar_target);
-            spacings_pass2<BS>(a, sh, s_warp);
-        }
-        bar_target += gridDim.x;
-        grid_barrier(a, bar_target);
-        // shared tail of both searches: gather the ancestors' states, restart weights, propagate
-        auto finish_pair = [&](int64_t p, const double *X0, const double *X1, int64_t a0, int64_t a1, long long g0,
-                               long long g1, bool write_A = true) {
-            double xp[2][D], base[2], x[2][D];
-#pragma unroll
-            for (int c = 0; c < D; c++) {                // Xp = X[A], component-wise (SoA)
-                xp[0][c] = __ldg(X0 + (size_t)c * n + a0);
-                xp[1][c] = __ldg(X1 + (size_t)c * n + a1);
-            }
-            if (APF) {   // core.py:302: lw = log_mean_exp(logetat, W) - logetat[A]
-                base[0] = reset_c - model_logeta<M>(model, kprev, xp[0]);
-                base[1] = reset_c - model_logeta<M>(model, kprev, xp[1]);
-            } else {     // Weights() then add(delta): lw = 0 + delta (shard mass if sharded)
-                base[0] = reset_c; base[1] = reset_c;
-            }
-            if (write_A) {
-                if (2 * p + 1 < n) *reinterpret_cast<longlong2 *>(a.A + 2 * p) = make_longlong2(g0, g1);
-                else a.A[2 * p] = g0;
-            }
-            double l[2], av[2];
-            if (zin == nullptr && vec_x && 2 * p + 1 < n) {       // complete pair, device normals: no bounds tests
-                double z[2][NZ];
-                tab_normals<NZ>(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t, z);
-                const bool odd = move_pair<M, FK, false>(model, k, xp, base, z, last_apf, x, l, av);
-#pragma unroll
-                for (int c = 0; c < D; c++) st2(Xo + (size_t)c * n + 2 * p, x[0][c], x[1][c]);
-                st2(lwo + 2 * p, l[0], l[1]);
-                if (!odd) acc_add_batch<2, D, true>(acc, l, x, mom);
-                else acc_add_batch<2, D, false>(acc, l, x, mom);
-            } else {
-                do_pair(io0, p, xp, base, x, l, av);
-                acc_add_batch<2, D>(acc, l, x, mom);
-            }
-            if (APF) lse3_add_batch<2>(aux, av);
-        };
-        if (count_path) {
-            // move pass of the counting path: every output verifies the scattered ancestor against the exact su_k
-            // (cdf[a-1] < su_k <= cdf[a], i.e. np.searchsorted's answer), walks if the hint is off, then gathers,
-            // propagates and reweights.  No tiles, no block barriers: a pair per thread, strided over the CTA's range.
-            const double M_ = (double)n;
-            // exact answer from any starting point: gallop to a bracket, then bisect (O(log distance) loads)
-            auto settle = [&](long long a0, double su) -> long long {
-                a0 = a0 < 0 ? 0 : (a0 > n - 1 ? n - 1 : a0);
-                long long lo_, hi_;                                  // answer in [lo_, hi_]: cdf[lo_-1] < su, cdf[hi_] >= su or hi_ = n-1
-                if (__ldcg(a.cdf + a0) < su) {                       // go up
-                    long long step = 1;
-                    lo_ = a0 + 1;
-                    hi_ = a0 + 1;
-                    while (hi_ < n - 1 && __ldcg(a.cdf + hi_) < su) { lo_ = hi_ + 1; hi_ += step; step <<= 1; }
-                    if (hi_ > n - 1) hi_ = n - 1;
-                } else {                                             // go down
-                    long long step = 1;
-                    hi_ = a0;
-                    lo_ = a0 - 1;
-                    while (lo_ >= 0 && __ldcg(a.cdf + lo_) >= su) { hi_ = lo_; lo_ -= step; step <<= 1; }
-                    lo_ = lo_ < 0 ? 0 : lo_ + 1;
-                }
-                while (lo_ < hi_) {                                  // first j in [lo_, hi_] with cdf[j] >= su
-                    const long long mid = lo_ + ((hi_ - lo_) >> 1);
-                    if (__ldcg(a.cdf + mid) < su) lo_ = mid + 1; else hi_ = mid;
-                }
-                return lo_;
-            };
-            constexpr int kR = kMovePairs;                          // pairs in flight per thread
-            // one round = kR pairs per thread, in three parts: the hints (A, written by the scan), the CDF entries that
-            // verify them, and verify + repair + gather + propagate
-            struct Hints { long long h[kR][2]; };
-            struct Cdf { double c0[kR][2], cm[kR][2], c1[kR][(SCHEME == SMCB_RS_STRATIFIED) ? 2 : 1]; };
-            auto ld_hints = [&](int64_t p0, Hints &H) {
-#pragma unroll
-                for (int r = 0; r < kR; r++) {
-                    const int64_t p = p0 + (int64_t)r * BS;
-                    H.h[r][0] = H.h[r][1] = 0;
-                    if (p < pend && 2 * p + 1 < n) {
-                        const longlong2 hh = __ldcg(reinterpret_cast<const longlong2 *>(a.A + 2 * p));
-                        H.h[r][0] = hh.x; H.h[r][1] = hh.y;
-                    } else if (p < pend) {
-                        H.h[r][0] = __ldcg(a.A + 2 * p);
-                    }
-                }
-            };
-            auto ld_cdf = [&](int64_t p0, const Hints &H, Cdf &Cc) {
-#pragma unroll
-                for (int r = 0; r < kR; r++) {
-                    const int64_t p = p0 + (int64_t)r * BS;
-#pragma unroll
-                    for (int q = 0; q < 2; q++) {                    // the two CDF entries that decide the hint
-                        long long hh = H.h[r][q];
-                        hh = hh < 0 ? 0 : (hh > n - 1 ? n - 1 : hh);
-                        const bool on = (p < pend) && (q == 0 || 2 * p + 1 < n);
-                        // (plain loads: this SM touches these lines for the first time in this launch, after the grid
-                        // barrier, so L1 cannot hold an older copy -- and neighbouring outputs reuse them)
-                        Cc.c0[r][q] = on ? a.cdf[hh] : 2.0;
-                        Cc.cm[r][q] = (on && hh > 0) ? a.cdf[hh - 1] : -1.0;
-                        // stratified: the hint answers k / N and su_k lies up to 1 / N further, so about half of the
-                        // outputs belong to the NEXT entry -- fetch it with the other two instead of walking
-                        if (SCHEME == SMCB_RS_STRATIFIED) Cc.c1[r][q] = (on && hh + 1 < n) ? a.cdf[hh + 1] : 2.0;
-                    }
-                }
-            };
-            auto process = [&](int64_t p0, const Hints &H, const Cdf &Cc) {
-                long long h[kR][2];
-                double su[kR][2];
-                bool valid[kR], two[kR], moved[kR];
-#pragma unroll
-                for (int r = 0; r < kR; r++) {
-                    const int64_t p = p0 + (int64_t)r * BS;
-                    moved[r] = false;
-                    valid[r] = p < pend;
-                    two[r] = valid[r] && (2 * p + 1 < n);
-                    grid_pair<SCHEME>(u_sys, a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t, uin, p, valid[r],
-                                      two[r], M_, su[r][0], su[r][1]);
-#pragma unroll
-                    for (int q = 0; q < 2; q++) {
-                        long long hh = H.h[r][q];
-                        hh = hh < 0 ? 0 : (hh > n - 1 ? n - 1 : hh);
-                        moved[r] = moved[r] || hh != H.h[r][q];
-                        h[r][q] = hh;
-                    }
-                }
-#pragma unroll
-                for (int r = 0; r < kR; r++) {
-#pragma unroll
-                    for (int q = 0; q < 2; q++) {
-                        const bool on = q == 0 ? valid[r] : two[r];
-                        bool ok = (Cc.cm[r][q] < su[r][q]) && (su[r][q] <= Cc.c0[r][q] || h[r][q] == n - 1);
-                        if (SCHEME == SMCB_RS_STRATIFIED) {
-                            if (on && !ok && Cc.c0[r][q] < su[r][q] && (su[r][q] <= Cc.c1[r][q] || h[r][q] + 1 == n - 1)) {
-                                h[r][q] += 1; moved[r] = true; ok = true;
-                            }
-                        }
-                        if (on && !ok && Cc.c0[r][q] < su[r][q] && h[r][q] + 1 < n) {
-                            // the hint is too low: ONE round trip for the next kWin entries (independent loads, mostly
-                            // one line) instead of a chain of dependent ones; the search below only runs past them
-                            constexpr int kWin = 6;
-                            const long long b = h[r][q] + 1;
-                            double wv[kWin];
-#pragma unroll
-                            for (int i = 0; i < kWin; i++) wv[i] = (b + i < n) ? __ldcg(a.cdf + b + i) : 2.0;
-                            int cnt = 0;
-#pragma unroll
-                            for (int i = 0; i < kWin; i++) cnt += (wv[i] < su[r][q]) ? 1 : 0;   // monotone CDF: a prefix
-                            if (cnt < kWin) {
-                                long long hn = b + cnt;
-                                h[r][q] = hn > n - 1 ? n - 1 : hn;
-                                moved[r] = true; ok = true;
-                            }
-                        }
-                        if (on && !ok) {
-                            h[r][q] = settle(h[r][q], su[r][q]);
-                            moved[r] = true;
-                        }
-                    }
-                    if (!two[r]) h[r][1] = h[r][0];
-                }
-#pragma unroll
-                for (int r = 0; r < kR; r++) {
-                    const int64_t p = p0 + (int64_t)r * BS;
-                    if (valid[r]) finish_pair(p, Xi, Xi, h[r][0], h[r][1], h[r][0], h[r][1], moved[r]);
-                }
-            };
-            constexpr int64_t kStep = (int64_t)kR * BS;
-            for (int64_t p0 = pstart + threadIdx.x; p0 < pend; p0 += kStep) {
-                Hints H;
-                Cdf Cc;
-                ld_hints(p0, H);
-                ld_cdf(p0, H, Cc);
-                process(p0, H, Cc);
-            }
-        } else if (SCHEME == SMCB_RS_MULTINOMIAL && !a.rs_global) {
-            // (every other scheme counts offspring when it resamples locally)
-            const double zlast = __ldcg(a.su + n);
-            int64_t lo = -1;
-            if (threadIdx.x == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_init_fence(); }
-            __syncthreads();
-            uint32_t phase0 = 0, phase1 = 0;
-            int buf = 0;
-            // thread 0: bring cdf[sb, sb + c) into buffer b (sb = lo_ rounded down to even => 16-byte aligned)
-            // by ONE TMA bulk copy (cp.async.bulk + mbarrier); the slice of tile i+1 is in flight while tile i
-            // propagates and reweights
-            auto issue = [&](int64_t lo_, int b) {
-                const int64_t sb = lo_ & ~(int64_t)1;
-                const int c = (int)((n - sb) < kStage ? (n - sb) : kStage);
-                const uint32_t bytes = (uint32_t)(c & ~1) * 8u;
-                double *dst = s_stage + (size_t)b * kStage;
-                if (c & 1) dst[c - 1] = __ldcg(a.cdf + sb + c - 1);      // odd tail (n odd, end of the array)
-                if (bytes) {
-                    mbar_arrive_expect_tx(&s_bar[b], bytes);
-                    tma_bulk_g2s(dst, a.cdf + sb, bytes, &s_bar[b]);
-                } else {
-                    mbar_arrive(&s_bar[b]);
-                }
-            };
-            for (int64_t pbase = pstart; pbase < pend; pbase += BS) {
-                const int64_t p = pbase + threadIdx.x;
-                const bool active = p < pend;
-                const int64_t k0 = 2 * pbase;                                       // first / last output of the tile
-                const int64_t ptop = pbase + BS < pend ? pbase + BS : pend;
-                const int64_t k1 = (2 * ptop < n ? 2 * ptop : n) - 1;
-                double su[2] = {2.0, 2.0};
-                if (active) {
-                    su[0] = __ldcg(a.su + 2 * p) / zlast;                   // resampling.py:537
-                    su[1] = (2 * p + 1 < n) ? __ldcg(a.su + 2 * p + 1) / zlast : 2.0;
-                    if (2 * p == k0) s_su[0] = su[0];
-                    if (2 * p == k1) s_su[1] = su[0];
-                    if (2 * p + 1 == k1) s_su[1] = su[1];
-                }
-                __syncthreads();
-                const double su_first = s_su[0], su_last = s_su[1];
-                if (lo < 0) {                                      // first tile of this block
-                    lo = block_lower_bound<BS>(a.cdf, 0, n, su_first);
-                    lo = lo < n - 1 ? lo : n - 1;
-                    if (threadIdx.x == 0) issue(lo, buf);
-                    __syncthreads();
-                }
-                // su is sorted, so the slice starts at `lo`
-                const int64_t sbase = lo & ~(int64_t)1;
-                const int cnt = (int)((n - sbase) < kStage ? (n - sbase) : kStage);
-                mbar_wait(&s_bar[buf], buf ? phase1 : phase0);
-                if (buf) phase1 ^= 1u; else phase0 ^= 1u;
-                const double *s_cdf = s_stage + (size_t)buf * kStage;
-                const bool covered = (sbase + cnt >= n) || (s_cdf[cnt - 1] >= su_last);
-                int64_t hi = lo;
-                if (!covered) hi = block_lower_bound<BS>(a.cdf, lo, n, su_last);   // rare: sparse mass
-                int64_t a0 = 0, a1 = 0;
-                if (active) {
-                    if (covered) {
-                        int l0 = (int)(lo - sbase), h0 = cnt;
-                        while (l0 < h0) { const int mid = (l0 + h0) >> 1; if (s_cdf[mid] < su[0]) l0 = mid + 1; else h0 = mid; }
-                        // su[1] >= su[0] and on average one CDF entry per output: walk forward a few
-                        // entries before falling back to bisection (same result as searchsorted)
-                        int l1 = l0, h1 = cnt;
-#pragma unroll
-                        for (int w = 0; w < 4; w++)
-                            if (l1 < cnt && s_cdf[l1] < su[1]) l1++;
-                        if (l1 < cnt && s_cdf[l1] < su[1]) {
-                            while (l1 < h1) { const int mid = (l1 + h1) >> 1; if (s_cdf[mid] < su[1]) l1 = mid + 1; else h1 = mid; }
-                        }
-                        a0 = sbase + l0;
-                        a1 = sbase + l1;
-                        if (2 * p == k1) s_hi = a0;
-                        if (2 * p + 1 == k1) s_hi = a1;
-                    } else {
-                        const int64_t hi1 = hi < n ? hi + 1 : n;
-                        a0 = lower_bound_cg(a.cdf, lo, hi1, su[0]);
-                        a1 = lower_bound_cg(a.cdf, a0, hi1, su[1]);
-                    }
-                }
-                __syncthreads();                                   // s_hi published; buffer buf^1 is free
-                const int64_t lo_next = covered ? (s_hi < n ? s_hi : n - 1) : (hi < n ? hi : n - 1);
-                if (pbase + BS < pend && threadIdx.x == 0) issue(lo_next, buf ^ 1);
-                if (active) {
-                    a0 = a0 < n - 1 ? a0 : n - 1;
-                    a1 = a1 < n - 1 ? a1 : n - 1;
-                    finish_pair(p, Xi, Xi, a0, a1, a0, a1);
-                }
-                lo = lo_next;
-                buf ^= 1;
-            }
-        } else {
-            // exact global resampling over particle shards (SURVEY.md section 8e, mode 2; resampling.py:599-610
-            // applied to the concatenation of all shards).  Output j of rank r is global offspring index_offset + j:
-            // its grid point su is located in the global CDF in two levels -- shard k with goff[k] <= su < goff[k+1]
-            // (offsets from the exchanged statistics, identical bits on every rank), then v = (su - goff[k]) / gpi[k]
-            // in shard k's own normalised CDF, read over NVLink -- and the ancestor's state is pulled from shard k's
-            // particle buffer.  First: tell every peer that this shard's CDF of step t is complete, and wait for theirs.
-            if (blockIdx.x == 0 && (int)threadIdx.x < a.world) {
-                __threadfence_system();
-                double *slot = a.mail_peer[threadIdx.x] + ((size_t)(t & 1) * a.world + a.rank) * kMailStride;
-                *reinterpret_cast<volatile double *>(slot + kMailScan) = (double)(t + 1);
-            }
-            if ((int)threadIdx.x < a.world)
-                wait_epoch(a.mail_local + ((size_t)(t & 1) * a.world + threadIdx.x) * kMailStride + kMailScan,
-                           (double)(t + 1), a.sync_timeout);
-            __syncthreads();
-            const int world = a.world;
-            const double M_ = (double)a.n_global;
-            double *s_cdf = s_stage;
-            int64_t lo = -1;
-            int lo_shard = -1;
-            for (int64_t pbase = pstart; pbase < pend; pbase += BS) {
-                const int64_t p = pbase + threadIdx.x;
-                const bool active = p < pend;                               // sharded filters have even n
-                const int64_t k0 = 2 * pbase;
-                const int64_t ptop = pbase + BS < pend ? pbase + BS : pend;
-                const int64_t k1 = 2 * ptop - 1;
-                double su[2] = {2.0, 2.0};
-                if (active) {
-                    const double g0 = (double)(a.index_offset + 2 * p);
-                    if (SCHEME == SMCB_RS_SYSTEMATIC) {
-                        su[0] = (u_sys + g0) / M_;
-                        su[1] = (u_sys + (g0 + 1.0)) / M_;
-                    } else {
-                        double u0, u1;
-                        if (uin) { u0 = uin[2 * p]; u1 = uin[2 * p + 1]; }
-                        else uniform_pair(a.key, (uint64_t)((a.index_offset >> 1) + p), (uint32_t)t, kPurposeUniform, u0, u1);
-                        su[0] = (u0 + g0) / M_;
-                        su[1] = (u1 + (g0 + 1.0)) / M_;
-                    }
-                    if (2 * p == k0) s_su[0] = su[0];
-                    if (2 * p + 1 == k1) s_su[1] = su[1];
-                }
-                __syncthreads();
-                const double su_first = s_su[0], su_last = s_su[1];
-                const int kf = shard_of(sh.goff, sh.gpi, world, su_first);
-                const int kl = shard_of(sh.goff, sh.gpi, world, su_last);
-                int ks[2] = {kf, kf};
-                int64_t an[2] = {0, 0};
-                if (kf == kl) {
-                    // the whole tile draws from one shard: staged search on that shard's CDF with the grid
-                    // points mapped into its local scale
-                    const double *cdf = a.pcdf[kf];
-                    const double off = sh.goff[kf], pi = sh.gpi[kf];
-                    const double v0 = fmin((su[0] - off) / pi, 1.0), v1 = fmin((su[1] - off) / pi, 1.0);
-                    const double v_first = fmin((su_first - off) / pi, 1.0), v_last = fmin((su_last - off) / pi, 1.0);
-                    if (lo < 0 || lo_shard != kf) lo = block_lower_bound<BS>(cdf, 0, n, v_first);
-                    if (lo > n - 1) lo = n - 1;
-                    lo_shard = kf;
-                    const int64_t sbase = lo & ~(int64_t)1;
-                    const int cnt = (int)((n - sbase) < kStage ? (n - sbase) : kStage);
-                    for (int i = 2 * threadIdx.x; i < cnt; i += 2 * BS) {
-                        if (i + 1 < cnt) *reinterpret_cast<double2 *>(&s_cdf[i]) = __ldcg(reinterpret_cast<const double2 *>(cdf + sbase + i));
-                        else s_cdf[i] = __ldcg(cdf + sbase + i);
-                    }
-                    __syncthreads();
-                    const bool covered = (sbase + cnt >= n) || (s_cdf[cnt - 1] >= v_last);
-                    int64_t hi = lo;
-                    if (!covered) hi = block_lower_bound<BS>(cdf, lo, n, v_last);
-                    if (active) {
-                        if (covered) {
-                            int l0 = (int)(lo - sbase), h0 = cnt;
-                            while (l0 < h0) { const int mid = (l0 + h0) >> 1; if (s_cdf[mid] < v0) l0 = mid + 1; else h0 = mid; }
-                            int l1 = l0, h1 = cnt;
-#pragma unroll
-                            for (int w = 0; w < 4; w++)
-                                if (l1 < cnt && s_cdf[l1] < v1) l1++;
-                            if (l1 < cnt && s_cdf[l1] < v1) {
-                                while (l1 < h1) { const int mid = (l1 + h1) >> 1; if (s_cdf[mid] < v1) l1 = mid + 1; else h1 = mid; }
-                            }
-                            an[0] = sbase + l0;
-                            an[1] = sbase + l1;
-                            if (2 * p + 1 == k1) s_hi = an[1];
-                        } else {
-                            const int64_t hi1 = hi < n ? hi + 1 : n;
-                            an[0] = lower_bound_cg(cdf, lo, hi1, v0);
-                            an[1] = lower_bound_cg(cdf, an[0], hi1, v1);
-                        }
-                    }
-                    __syncthreads();
-                    lo = covered ? (s_hi < n ? s_hi : n - 1) : (hi < n ? hi : n - 1);
-                } else {
-                    // the tile straddles a shard boundary (at most world - 1 tiles per rank): plain searches
-                    if (active) {
-#pragma unroll
-                        for (int j = 0; j < 2; j++) {
-                            ks[j] = shard_of(sh.goff, sh.gpi, world, su[j]);
-                            const double v = fmin((su[j] - sh.goff[ks[j]]) / sh.gpi[ks[j]], 1.0);
-                            an[j] = lower_bound_cg(a.pcdf[ks[j]], 0, n, v);
-                        }
-                    }
-                    lo = -1;
-                }
-                if (active) {
-                    const int64_t a0 = an[0] < n - 1 ? an[0] : n - 1, a1 = an[1] < n - 1 ? an[1] : n - 1;
-                    // ancestors are GLOBAL particle indices
-                    finish_pair(p, a.pX[ks[0]][cur], a.pX[ks[1]][cur], a0, a1, (long long)ks[0] * n + a0,
-                                (long long)ks[1] * n + a1);
-                }
-                __syncthreads();       // s_su / s_hi / s_cdf are rewritten by the next tile
-            }
-        }
+        resample_scan<M, FK, SCHEME>(model, a, e, dec, u_sys, sh, s_stage, s_warp);
+        if (SCHEME != SMCB_RS_MULTINOMIAL && !a.rs_global)
+            move_counted<M, FK, SCHEME>(model, a, e, dec.reset_c, u_sys, uin, acc, aux);
+        else if (SCHEME == SMCB_RS_MULTINOMIAL && !a.rs_global)
+            move_tiles<M, FK>(model, a, e, dec.reset_c, acc, aux, s_stage, s_su, s_bar, s_hi);
+        else
+            move_global<M, FK, SCHEME>(model, a, e, dec.reset_c, u_sys, uin, acc, aux, sh, s_stage, s_su, s_hi);
     }
-step_done:
-    write_partial<D, APF, BS>(a, t, acc, aux, mom, sh, s_stage, n_slab);
-    if (fuse)   // (acc, aux: still empty -- the streaming branch keeps its statistics in the slab records)
-        write_partial<D, APF, BS>(a, t + 1, acc, aux, mom, sh, a.fuse_slab + (size_t)blockIdx.x * StepCfg<M>::kSlabDoubles,
+    write_partial<D, APF, BS>(a, t, acc, aux, e.mom, sh, s_stage, n_slab);
+    if (fuse)   // (acc, aux: still empty -- the streaming pass keeps its statistics in the slab records)
+        write_partial<D, APF, BS>(a, t + 1, acc, aux, e.mom, sh, a.fuse_slab + (size_t)blockIdx.x * StepCfg<M>::kSlabDoubles,
                                   n_slab);
 }
 

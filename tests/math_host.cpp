@@ -1,5 +1,6 @@
 // Host build of particles_b200/csrc/smcb_math.cuh (the step kernel's fp64 exp / log / sincos / batch
-// log-sum-exp) and smcb_models.cuh (the model / Feynman-Kac maps of the fused step kernel) so that their
+// log-sum-exp), smcb_models.cuh (the model / Feynman-Kac maps of the fused step kernel) and the step kernel's in-tile
+// CDF search of smcb_search.cuh so that their
 // ALGORITHMS can be checked on the CPU against NumPy / mpmath and against the oracle
 // (tests/test_math_host.py, tests/test_models_host.py).  CUDA intrinsics are restated bit-for-bit below; compile with
 // -ffp-contract=off so that only the explicit fma() calls fuse, as nvcc -fmad=false does.
@@ -50,6 +51,7 @@ static inline void philox4x32_10k(uint32_t, uint32_t, uint32_t, uint32_t, const 
 }  // namespace smcb
 #include "smcb_math.cuh"
 #include "smcb_models.cuh"
+#include "smcb_search.cuh"
 
 namespace {
 using namespace smcb;
@@ -154,5 +156,10 @@ void mh_lse3(const double *v, long n, double *out3) {
     for (; i + 4 <= n; i += 4) { const double b[4] = {v[i], v[i + 1], v[i + 2], v[i + 3]}; smcb::lse3_add_batch<4>(a, b); }
     for (; i < n; i++) { const double b[1] = {v[i]}; smcb::lse3_add_batch<1>(a, b); }
     out3[0] = a.m; out3[1] = a.s; out3[2] = a.q;
+}
+// the step kernel's in-tile search: for each query i, the answers for keys v[2i] <= v[2i+1] on the slice s[0, cnt)
+// searched from l0[i]
+void mh_tile_search(const double *s, int cnt, const int *l0, const double *v, long m, int *out) {
+    for (long i = 0; i < m; i++) smcb::tile_search(s, l0[i], cnt, v[2 * i], v[2 * i + 1], out[2 * i], out[2 * i + 1]);
 }
 }

@@ -139,6 +139,38 @@ def test_box_muller_and_lse3(mh):
     np.testing.assert_allclose(out[1:], [e.sum(), (e * e).sum()], rtol=1e-13)
 
 
+def test_tile_search():
+    """The in-tile CDF search of the step kernel's multinomial and global-resampling move passes
+    (smcb_search.cuh tile_search) against np.searchsorted(slice, v, 'left'): slices with ties and flat runs of zero
+    mass, keys below the first and above the last entry, slices of 1 and 2 entries, and start offsets up to the
+    first key's answer (at cnt when every entry lies below it)."""
+    lib = build_math_host()
+    r = np.random.RandomState(6)
+    for trial in range(400):
+        cnt = [1, 2, 3, 5, 8, 64, 4096][trial % 7]
+        steps = r.exponential(1.0, cnt) * (r.rand(cnt) < 0.6)          # zero steps: ties / flat runs
+        if trial % 5 == 0:
+            steps[r.randint(0, cnt):] = 0.0                               # a long flat tail
+        s = np.cumsum(steps) + r.uniform(-1.0, 1.0)
+        lo, hi = s[0] - 1.0, s[-1] + 1.0
+        m = 300
+        v0 = np.concatenate([r.uniform(lo, hi, m - 20), s[r.randint(0, cnt, 10)], [lo - 5.0] * 5, [hi + 5.0] * 5])
+        gap = np.where(r.rand(m) < 0.5, r.exponential(2.0 * (hi - lo) / cnt, m), 0.0)
+        v1 = v0 + gap * (r.rand(m) < 0.9) + (hi - lo + 10.0) * (r.rand(m) < 0.05)     # some far past the slice
+        eq = r.rand(m) < 0.1
+        v1[eq] = v0[eq]                                                   # both outputs on one key
+        want0, want1 = np.searchsorted(s, v0, "left"), np.searchsorted(s, v1, "left")
+        l0 = (r.rand(m) * (want0 + 1)).astype(np.int32)
+        near = r.rand(m) < 0.3
+        l0[near] = want0[near]                                            # start at the answer (up to cnt)
+        v = np.ascontiguousarray(np.stack([v0, v1], axis=1))
+        out = np.empty((m, 2), dtype=np.int32)
+        lib.mh_tile_search(s.ctypes.data_as(C.c_void_p), C.c_int(cnt), l0.ctypes.data_as(C.c_void_p),
+                           v.ctypes.data_as(C.c_void_p), C.c_long(m), out.ctypes.data_as(C.c_void_p))
+        assert np.array_equal(out[:, 0], want0), (cnt, trial)
+        assert np.array_equal(out[:, 1], want1), (cnt, trial)
+
+
 def test_sqrt_and_tables():
     """tsqrt_pos (reciprocal-square-root seed truncated to what MUFU.RSQ64H delivers + one third-order step) and
     the lookup tables themselves against mpmath."""
