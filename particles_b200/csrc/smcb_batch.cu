@@ -294,32 +294,24 @@ static int batch_one(smcb_ctx *c, const smcb_batch_desc &d, int64_t *out) {
 
 template <class M, int FK>
 static int batch_scheme(smcb_ctx *c, const smcb_batch_desc &d, int64_t *out) {
-    switch (d.scheme) {
-        case SMCB_RS_SYSTEMATIC: return batch_one<M, FK, SMCB_RS_SYSTEMATIC>(c, d, out);
-        case SMCB_RS_STRATIFIED: return batch_one<M, FK, SMCB_RS_STRATIFIED>(c, d, out);
-        case SMCB_RS_MULTINOMIAL: return batch_one<M, FK, SMCB_RS_MULTINOMIAL>(c, d, out);
-        default:
-            set_error("batched filter: resampling scheme %d is not built", d.scheme);
-            return SMCB_ENOSYS;
-    }
+    bool built = false;
+    const int rc = with_scheme(d.scheme, [&](auto scheme) {
+        built = true;
+        return batch_one<M, FK, decltype(scheme)::value>(c, d, out);
+    });
+    if (!built) set_error("batched filter: resampling scheme %d is not built", d.scheme);
+    return rc;
 }
 
 template <class M>
 static int batch_fk(smcb_ctx *c, const smcb_batch_desc &d, int64_t *out) {
-    switch (d.fk) {
-        case SMCB_FK_BOOTSTRAP: return batch_scheme<M, SMCB_FK_BOOTSTRAP>(c, d, out);
-        default: break;
-    }
-    if constexpr (M::has_proposal) {
-        switch (d.fk) {
-            case SMCB_FK_GUIDED: return batch_scheme<M, SMCB_FK_GUIDED>(c, d, out);
-            case SMCB_FK_APF: return batch_scheme<M, SMCB_FK_APF>(c, d, out);
-            case SMCB_FK_AUXBOOT: return batch_scheme<M, SMCB_FK_AUXBOOT>(c, d, out);
-            default: break;
-        }
-    }
-    set_error("batched filter: Feynman-Kac kind %d is not built for model %d", d.fk, d.model);
-    return SMCB_ENOSYS;
+    bool built = false;
+    const int rc = with_fk<M>(d.fk, [&](auto fk) {
+        built = true;
+        return batch_scheme<M, decltype(fk)::value>(c, d, out);
+    });
+    if (!built) set_error("batched filter: Feynman-Kac kind %d is not built for model %d", d.fk, d.model);
+    return rc;
 }
 
 static int batch_dispatch(smcb_ctx *c, const smcb_batch_desc *dp, int64_t *out) {
@@ -337,17 +329,18 @@ static int batch_dispatch(smcb_ctx *c, const smcb_batch_desc *dp, int64_t *out) 
         SMCB_REQUIRE(d.seed && d.essrmin && d.params && d.data && d.X && d.lw && d.A && d.summaries,
                      "smcb_batch: NULL buffer");
     }
-    switch (d.model) {
-        case SMCB_MODEL_STOCHVOL: return batch_fk<StochVolM>(c, d, out);
-        case SMCB_MODEL_LINGAUSS: return batch_fk<LinGaussM>(c, d, out);
-        case SMCB_MODEL_GORDON: return batch_fk<GordonM>(c, d, out);
-        case SMCB_MODEL_THETALOGISTIC: return batch_fk<ThetaLogisticM>(c, d, out);
-        case SMCB_MODEL_DISCRETECOX: return batch_fk<DiscreteCoxM>(c, d, out);
-        case SMCB_MODEL_STOCHVOLLEV: return batch_fk<StochVolLevM>(c, d, out);
-        default:
-            set_error("batched filter: model id %d is not built", d.model);
+    bool built = false;
+    const int rc = with_model(d.model, d.dim, [&](auto m) {
+        using M = decltype(m);
+        if constexpr (M::D == 1) {
+            built = true;
+            return batch_fk<M>(c, d, out);
+        } else {
             return SMCB_ENOSYS;
-    }
+        }
+    });
+    if (!built) set_error("batched filter: model id %d is not built", d.model);
+    return rc;
 }
 
 }  // namespace smcb

@@ -1,26 +1,38 @@
-// smcb_filter.cu -- host side of the fused filter (C-ABI entry points) + the 1-D model family.
-// The kernels live in smcb_step.cuh; the d-dimensional models are instantiated in
-// smcb_filter_nd.cu so that the two translation units compile in parallel.
+// smcb_filter.cu -- host side of the fused filter (C-ABI entry points) + the kernels of StochVol and LinearGauss.
+// The kernels live in smcb_step.cuh; the other models are instantiated in smcb_filter_1d.cu and smcb_filter_nd.cu
+// so that the three translation units compile in parallel.
 #include <stdlib.h>
 
 #include "smcb_step.cuh"
 
-int smcb_bind_nd(smcb_filter *f);      // smcb_filter_nd.cu
-int smcb_bind_1d_more(smcb_filter *f); // smcb_filter_1d.cu
+extern template int bind_fk<GordonM>(smcb_filter *);           // smcb_filter_1d.cu
+extern template int bind_fk<ThetaLogisticM>(smcb_filter *);
+extern template int bind_fk<DiscreteCoxM>(smcb_filter *);
+extern template int bind_fk<StochVolLevM>(smcb_filter *);
+extern template int bind_fk<BearingsM>(smcb_filter *);         // smcb_filter_nd.cu
+extern template int bind_fk<MvLinGaussM<2>>(smcb_filter *);
+extern template int bind_fk<MvLinGaussM<3>>(smcb_filter *);
+extern template int bind_fk<MvLinGaussM<4>>(smcb_filter *);
 
-static int smcb_bind_1d(smcb_filter *f) {
+// bind_fk<M> for the model of (desc.model, desc.dim); a model whose state dimension is not dim is not bound
+static int filter_bind(smcb_filter *f) {
     const smcb_filter_desc *d = &f->desc;
-    switch (d->model) {
-        case SMCB_MODEL_STOCHVOL: return bind_fk<StochVolM>(f);
-        case SMCB_MODEL_LINGAUSS: return bind_fk<LinGaussM>(f);
-        case SMCB_MODEL_GORDON:
-        case SMCB_MODEL_THETALOGISTIC:
-        case SMCB_MODEL_DISCRETECOX:
-        case SMCB_MODEL_STOCHVOLLEV: return smcb_bind_1d_more(f);
-        default:
-            set_error("fused filter: model id %d is not available in the fused 1-D family", d->model);
-            return SMCB_ENOSYS;
+    bool bound = false;
+    const int rc = with_model(d->model, d->dim, [&](auto m) {
+        using M = decltype(m);
+        if (M::D != d->dim) return SMCB_ENOSYS;
+        bound = true;
+        return bind_fk<M>(f);
+    });
+    if (bound) return rc;
+    if (d->dim != 1 && d->model == SMCB_MODEL_BEARINGS) {
+        set_error("fused BearingsOnly: state dimension must be 4");
+        return SMCB_EINVAL;
     }
+    if (d->dim == 1) set_error("fused filter: model id %d is not available in the fused 1-D family", d->model);
+    else if (d->model == SMCB_MODEL_MVLINGAUSS) set_error("fused MVLinearGauss: dx must be 2, 3 or 4 (got %d)", d->dim);
+    else set_error("fused filter: model id %d has no d-dimensional kernel", d->model);
+    return SMCB_ENOSYS;
 }
 
 static int filter_setup(smcb_filter *f, smcb_ctx *c, const smcb_filter_desc *d);
@@ -58,7 +70,7 @@ static bool env_flag(const char *name, bool dflt) {
 }
 
 static int filter_setup(smcb_filter *f, smcb_ctx *c, const smcb_filter_desc *d) {
-    int rc = (d->dim == 1) ? smcb_bind_1d(f) : smcb_bind_nd(f);
+    int rc = filter_bind(f);
     if (rc) return rc;
 
     const int64_t n = d->n;

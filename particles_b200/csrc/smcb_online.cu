@@ -8,6 +8,7 @@
 //   PHI_*      the update of Phi from the draws / weights and the user's psi, in a fixed summation order.
 // Randomness: Philox keyed by (seed, t, draw j, trial, purpose): the draws depend on the seed only, never on the
 // launch geometry or on other API calls.
+#include "smcb_dispatch.cuh"
 #include "smcb_smooth.cuh"
 
 using namespace smcb;
@@ -280,12 +281,6 @@ __global__ void __launch_bounds__(kBlock) k_phi_on2(smcb_online_desc d) {
     }
 }
 
-template <class K>
-int set_smem(K kern, size_t bytes) {
-    SMCB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    return SMCB_OK;
-}
-
 template <class M>
 int run_model(smcb_ctx *c, const smcb_online_desc &d) {
     SMCB_REQUIRE(d.dim == M::D, "smcb_online_smooth: dim %d does not match the model's %d", (int)d.dim, M::D);
@@ -339,21 +334,11 @@ extern "C" int smcb_online_smooth(smcb_ctx *c, const smcb_online_desc *dp) {
         SMCB_REQUIRE(d.omega && d.rows >= 1 && d.row0 >= 0 && d.row0 + d.rows <= d.N,
                      "smcb_online_smooth: bad ON2 rows [%lld, +%lld)", (long long)d.row0, (long long)d.rows);
     }
-    switch (d.model) {
-        case SMCB_MODEL_STOCHVOL: return run_model<StochVolM>(c, d);
-        case SMCB_MODEL_LINGAUSS: return run_model<LinGaussM>(c, d);
-        case SMCB_MODEL_GORDON: return run_model<GordonM>(c, d);
-        case SMCB_MODEL_THETALOGISTIC: return run_model<ThetaLogisticM>(c, d);
-        case SMCB_MODEL_DISCRETECOX: return run_model<DiscreteCoxM>(c, d);
-        case SMCB_MODEL_STOCHVOLLEV: return run_model<StochVolLevM>(c, d);
-        case SMCB_MODEL_BEARINGS: return run_model<BearingsM>(c, d);
-        case SMCB_MODEL_MVLINGAUSS:
-            if (d.dim == 2) return run_model<MvLinGaussM<2>>(c, d);
-            if (d.dim == 3) return run_model<MvLinGaussM<3>>(c, d);
-            if (d.dim == 4) return run_model<MvLinGaussM<4>>(c, d);
-            break;
-        default: break;
-    }
-    set_error("smcb_online_smooth: no transition density for model %d, dim %d", (int)d.model, (int)d.dim);
-    return SMCB_ENOSYS;
+    bool known = false;
+    const int rc = with_model(d.model, d.dim, [&](auto m) {
+        known = true;
+        return run_model<decltype(m)>(c, d);
+    });
+    if (!known) set_error("smcb_online_smooth: no transition density for model %d, dim %d", (int)d.model, (int)d.dim);
+    return rc;
 }

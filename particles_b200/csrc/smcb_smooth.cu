@@ -10,6 +10,7 @@
 //           warp-cooperative exact O(N) draw for every lane still rejected.
 // Randomness: Philox keyed by (context seed, API call, trajectory m, time t, trial, purpose): results depend on the
 // seed only, never on the launch geometry.
+#include "smcb_dispatch.cuh"
 #include "smcb_smooth.cuh"
 
 using namespace smcb;
@@ -280,12 +281,6 @@ __global__ void __launch_bounds__(kBlock) k_bs_gather(smcb_smooth_desc d) {
     }
 }
 
-template <class K>
-int set_smem(K kern, size_t bytes) {
-    SMCB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    return SMCB_OK;
-}
-
 template <class M>
 int run_model(smcb_ctx *c, const smcb_smooth_desc &d) {
     SMCB_REQUIRE(d.dim == M::D, "smcb_backward_sample: dim %d does not match the model's %d", (int)d.dim, M::D);
@@ -345,21 +340,11 @@ extern "C" int smcb_backward_sample(smcb_ctx *c, const smcb_smooth_desc *dp) {
                      "smcb_backward_sample: reject needs the CDFs");
         SMCB_REQUIRE((d.prop == nullptr) == (d.lu == nullptr), "smcb_backward_sample: prop and lu go together");
     }
-    switch (d.model) {
-        case SMCB_MODEL_STOCHVOL: return run_model<StochVolM>(c, d);
-        case SMCB_MODEL_LINGAUSS: return run_model<LinGaussM>(c, d);
-        case SMCB_MODEL_GORDON: return run_model<GordonM>(c, d);
-        case SMCB_MODEL_THETALOGISTIC: return run_model<ThetaLogisticM>(c, d);
-        case SMCB_MODEL_DISCRETECOX: return run_model<DiscreteCoxM>(c, d);
-        case SMCB_MODEL_STOCHVOLLEV: return run_model<StochVolLevM>(c, d);
-        case SMCB_MODEL_BEARINGS: return run_model<BearingsM>(c, d);
-        case SMCB_MODEL_MVLINGAUSS:
-            if (d.dim == 2) return run_model<MvLinGaussM<2>>(c, d);
-            if (d.dim == 3) return run_model<MvLinGaussM<3>>(c, d);
-            if (d.dim == 4) return run_model<MvLinGaussM<4>>(c, d);
-            break;
-        default: break;
-    }
-    set_error("smcb_backward_sample: no transition density for model %d, dim %d", (int)d.model, (int)d.dim);
-    return SMCB_ENOSYS;
+    bool known = false;
+    const int rc = with_model(d.model, d.dim, [&](auto m) {
+        known = true;
+        return run_model<decltype(m)>(c, d);
+    });
+    if (!known) set_error("smcb_backward_sample: no transition density for model %d, dim %d", (int)d.model, (int)d.dim);
+    return rc;
 }

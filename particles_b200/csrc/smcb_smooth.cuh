@@ -1,6 +1,6 @@
 // smcb_smooth.cuh -- device pieces shared by the backward samplers (smcb_smooth.cu) and the on-line smoothers
 // (smcb_online.cu): Philox uniforms of a draw, inverse-CDF multinomial draw, online log-sum-exp, the warp-cooperative
-// exact draw and one rejection trial.
+// exact draw and one rejection trial; on the host, the shared-memory attribute of a launch.
 //
 // The history-reading helpers are templated on the descriptor.  A descriptor `d` provides the pointer tables
 // d.X[t] and d.lw[t], the element strides d.x_stride_n / d.x_stride_c, the sizes d.N (particles at t), d.M (draws)
@@ -150,5 +150,12 @@ __device__ __forceinline__ bool reject_trial(const M &m, const TransDensity<M> &
 
 // trials each lane runs on its own before the warp serves the lanes still rejected together
 constexpr int64_t kSoloTrials = 4;
+
+// host: lets launches of `kern` use `bytes` of dynamic shared memory
+template <class K>
+int set_smem(K kern, size_t bytes) {
+    SMCB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    return SMCB_OK;
+}
 
 }  // namespace smcb

@@ -29,6 +29,7 @@
 #include <type_traits>
 
 #include "smcb_common.cuh"
+#include "smcb_dispatch.cuh"
 #include "smcb_math.cuh"
 #include "smcb_models.cuh"
 #include "smcb_scan.cuh"
@@ -2137,34 +2138,32 @@ static int bind_one(smcb_filter *f) {
 
 template <class M, int FK>
 static int bind_scheme(smcb_filter *f) {
-    switch (f->desc.scheme) {
-        case SMCB_RS_SYSTEMATIC: return bind_one<M, FK, SMCB_RS_SYSTEMATIC>(f);
-        case SMCB_RS_STRATIFIED: return bind_one<M, FK, SMCB_RS_STRATIFIED>(f);
-        case SMCB_RS_MULTINOMIAL: return bind_one<M, FK, SMCB_RS_MULTINOMIAL>(f);
-        default:
-            set_error("fused filter: resampling scheme %d is not fused (use systematic, stratified or "
-                      "multinomial, or the unfused path)", f->desc.scheme);
-            return SMCB_ENOSYS;
-    }
+    bool fused = false;
+    const int rc = with_scheme(f->desc.scheme, [&](auto scheme) {
+        fused = true;
+        return bind_one<M, FK, decltype(scheme)::value>(f);
+    });
+    if (!fused)
+        set_error("fused filter: resampling scheme %d is not fused (use systematic, stratified or "
+                  "multinomial, or the unfused path)", f->desc.scheme);
+    return rc;
 }
 
+// Binds the kernels of model M.  Each model's kernels are compiled in one translation unit only: smcb_filter.cu
+// dispatches on the model id and instantiates StochVol and LinearGauss; the other models' bind_fk<M> are declared
+// extern template there and instantiated explicitly in smcb_filter_1d.cu and smcb_filter_nd.cu.
 template <class M>
-static int bind_fk(smcb_filter *f) {
-    switch (f->desc.fk) {
-        case SMCB_FK_BOOTSTRAP: return bind_scheme<M, SMCB_FK_BOOTSTRAP>(f);
-        case SMCB_FK_GUIDED:
-            if (!M::has_proposal) break;
-            return bind_scheme<M, SMCB_FK_GUIDED>(f);
-        case SMCB_FK_APF:
-            if (!M::has_proposal) break;
-            return bind_scheme<M, SMCB_FK_APF>(f);
-        case SMCB_FK_AUXBOOT:
-            if (!M::has_proposal) break;
-            return bind_scheme<M, SMCB_FK_AUXBOOT>(f);
-        default:
-            set_error("fused filter: unknown Feynman-Kac kind %d", f->desc.fk);
-            return SMCB_EINVAL;
+int bind_fk(smcb_filter *f) {
+    if (f->desc.fk < SMCB_FK_BOOTSTRAP || f->desc.fk > SMCB_FK_AUXBOOT) {
+        set_error("fused filter: unknown Feynman-Kac kind %d", f->desc.fk);
+        return SMCB_EINVAL;
     }
+    bool offered = false;
+    const int rc = with_fk<M>(f->desc.fk, [&](auto fk) {
+        offered = true;
+        return bind_scheme<M, decltype(fk)::value>(f);
+    });
+    if (offered) return rc;
     // the reference raises NotImplementedError from StateSpaceModel.proposal / logeta
     set_error("fused filter: model %d implements no proposal/logeta (Feynman-Kac kind %d)",
               f->desc.model, f->desc.fk);

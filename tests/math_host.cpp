@@ -1,6 +1,7 @@
 // Host build of particles_b200/csrc/smcb_math.cuh (the step kernel's fp64 exp / log / sincos / batch
-// log-sum-exp), smcb_models.cuh (the model / Feynman-Kac maps of the fused step kernel) and the step kernel's in-tile
-// CDF search of smcb_search.cuh so that their
+// log-sum-exp), smcb_models.cuh (the model / Feynman-Kac maps of the fused step kernel), the library's table of
+// (model, Feynman-Kac kind) combinations in smcb_dispatch.cuh and the step kernel's in-tile CDF search of
+// smcb_search.cuh so that their
 // ALGORITHMS can be checked on the CPU against NumPy / mpmath and against the oracle
 // (tests/test_math_host.py, tests/test_models_host.py).  CUDA intrinsics are restated bit-for-bit below; compile with
 // -ffp-contract=off so that only the explicit fma() calls fuse, as nvcc -fmad=false does.
@@ -51,6 +52,7 @@ static inline void philox4x32_10k(uint32_t, uint32_t, uint32_t, uint32_t, const 
 }  // namespace smcb
 #include "smcb_math.cuh"
 #include "smcb_models.cuh"
+#include "smcb_dispatch.cuh"
 #include "smcb_search.cuh"
 
 namespace {
@@ -90,40 +92,23 @@ void step_all(const double *params, const StepK &k, const double *xp, const doub
         if (leta) leta[i] = model_logeta<M>(m, k, xi);
     }
 }
-template <class M>
-int step_fk(int fk, const double *params, const StepK &k, const double *xp, const double *z, long n, double *x,
-            double *delta, double *leta) {
-    if (fk == SMCB_FK_BOOTSTRAP) { step_all<M, SMCB_FK_BOOTSTRAP>(params, k, xp, z, n, x, delta, nullptr); return 0; }
-    if constexpr (M::has_proposal) {
-        if (fk == SMCB_FK_GUIDED) { step_all<M, SMCB_FK_GUIDED>(params, k, xp, z, n, x, delta, nullptr); return 0; }
-        if (fk == SMCB_FK_APF) { step_all<M, SMCB_FK_APF>(params, k, xp, z, n, x, delta, leta); return 0; }
-        if (fk == SMCB_FK_AUXBOOT) { step_all<M, SMCB_FK_AUXBOOT>(params, k, xp, z, n, x, delta, leta); return 0; }
-    }
-    return -3;
-}
 }  // namespace
 
 extern "C" {
-// returns 0, or -3 when the (model, Feynman-Kac kind, dimension) combination has no fused kernel
+// returns 0, or -3 (SMCB_ENOSYS) when the (model, Feynman-Kac kind, dimension) combination has no fused kernel:
+// the library's own table, smcb_dispatch.cuh, decides
 int mh_model_step(int model, int fk, int dim, const double *params, const double *data, long T, int dy,
                   const double *sc, long t, const double *xp, const double *z, long n, double *x, double *delta,
                   double *leta) {
     const StepK k = make_step(data, T, dy, sc, t);
-    switch (model) {
-        case SMCB_MODEL_STOCHVOL: return step_fk<StochVolM>(fk, params, k, xp, z, n, x, delta, leta);
-        case SMCB_MODEL_LINGAUSS: return step_fk<LinGaussM>(fk, params, k, xp, z, n, x, delta, leta);
-        case SMCB_MODEL_GORDON: return step_fk<GordonM>(fk, params, k, xp, z, n, x, delta, leta);
-        case SMCB_MODEL_THETALOGISTIC: return step_fk<ThetaLogisticM>(fk, params, k, xp, z, n, x, delta, leta);
-        case SMCB_MODEL_DISCRETECOX: return step_fk<DiscreteCoxM>(fk, params, k, xp, z, n, x, delta, leta);
-        case SMCB_MODEL_STOCHVOLLEV: return step_fk<StochVolLevM>(fk, params, k, xp, z, n, x, delta, leta);
-        case SMCB_MODEL_BEARINGS: return step_fk<BearingsM>(fk, params, k, xp, z, n, x, delta, leta);
-        case SMCB_MODEL_MVLINGAUSS:
-            if (dim == 2) return step_fk<MvLinGaussM<2>>(fk, params, k, xp, z, n, x, delta, leta);
-            if (dim == 3) return step_fk<MvLinGaussM<3>>(fk, params, k, xp, z, n, x, delta, leta);
-            if (dim == 4) return step_fk<MvLinGaussM<4>>(fk, params, k, xp, z, n, x, delta, leta);
-            return -3;
-        default: return -3;
-    }
+    return with_model(model, dim, [&](auto m) {
+        using M = decltype(m);
+        return with_fk<M>(fk, [&](auto kind) {
+            constexpr int FK = decltype(kind)::value;
+            step_all<M, FK>(params, k, xp, z, n, x, delta, FkTraits<FK>::apf ? leta : nullptr);
+            return 0;
+        });
+    });
 }
 
 static double g_tables[smcb::kMathTabDoubles];

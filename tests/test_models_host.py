@@ -99,3 +99,15 @@ def test_unfused_combinations_answer_enosys(mh):
     rc = mh.mh_model_step(4, 1, 4, ptr(np.zeros(16)), ptr(data), C.c_long(2), 1, None, C.c_long(0), None, ptr(z),
                           C.c_long(4), ptr(out), ptr(d), None)          # BearingsOnly has no proposal
     assert rc == -3
+
+    def step(model, fk, dim):
+        return mh.mh_model_step(model, fk, dim, ptr(np.zeros(64)), ptr(data), C.c_long(2), 1, None, C.c_long(0), None,
+                                ptr(z), C.c_long(4), ptr(out), ptr(d), ptr(np.empty(4)))
+
+    assert step(8, 0, 1) == -3 and step(-1, 0, 1) == -3                 # unknown model ids
+    assert step(0, 4, 1) == -3                                          # unknown Feynman-Kac kind
+    assert step(5, 0, 5) == -3 and step(5, 0, 1) == -3                  # MVLinearGauss is fused for dx = 2, 3, 4
+    # Gordon, ThetaLogistic, BearingsOnly, DiscreteCox, StochVolLeverage: no proposal / logeta, so bootstrap only
+    for model, dim in ((2, 1), (3, 1), (4, 4), (6, 1), (7, 1)):
+        for fk in (1, 2, 3):
+            assert step(model, fk, dim) == -3, (model, fk)

@@ -28,20 +28,9 @@ int mh_trans_logpdf(int model, int dim, const double *params, const double *sc, 
     StepK k{};
     k.t = t;
     k.sc0 = sc ? sc[t] : 0.0;
-    switch (model) {
-        case SMCB_MODEL_STOCHVOL: trans_all<StochVolM>(params, k, xp, x, n, out); return 0;
-        case SMCB_MODEL_LINGAUSS: trans_all<LinGaussM>(params, k, xp, x, n, out); return 0;
-        case SMCB_MODEL_GORDON: trans_all<GordonM>(params, k, xp, x, n, out); return 0;
-        case SMCB_MODEL_THETALOGISTIC: trans_all<ThetaLogisticM>(params, k, xp, x, n, out); return 0;
-        case SMCB_MODEL_DISCRETECOX: trans_all<DiscreteCoxM>(params, k, xp, x, n, out); return 0;
-        case SMCB_MODEL_STOCHVOLLEV: trans_all<StochVolLevM>(params, k, xp, x, n, out); return 0;
-        case SMCB_MODEL_BEARINGS: trans_all<BearingsM>(params, k, xp, x, n, out); return 0;
-        case SMCB_MODEL_MVLINGAUSS:
-            if (dim == 2) { trans_all<MvLinGaussM<2>>(params, k, xp, x, n, out); return 0; }
-            if (dim == 3) { trans_all<MvLinGaussM<3>>(params, k, xp, x, n, out); return 0; }
-            if (dim == 4) { trans_all<MvLinGaussM<4>>(params, k, xp, x, n, out); return 0; }
-            return -3;
-        default: return -3;
-    }
+    return with_model(model, dim, [&](auto m) {
+        trans_all<decltype(m)>(params, k, xp, x, n, out);
+        return 0;
+    });
 }
 }
