@@ -442,6 +442,65 @@ int smcb_batch_plan(smcb_ctx *ctx, const smcb_batch_desc *desc, int64_t out[2]);
 /* one launch on the context's stream, no host sync */
 int smcb_batch_run(smcb_ctx *ctx, const smcb_batch_desc *desc);
 
+/* ---------------------------------------------------------------------------
+ * filter bank (SMC^2, particles/smc_samplers.py:1038-1167): R resumable filters of one 1-D fused model, Feynman-Kac
+ * kind, scheme, N and data, each with its own model constants and Philox key, kept in device rows between launches
+ * (csrc/smcb_bank.cu).  The geometry and the step body are those of the batched filters: advancing a filter over
+ * [0, t) and then [t, t1) gives the bits of advancing it over [0, t1) in one call, and filter r draws what the
+ * batched run (and the single filter) with seed key[r] draws.  Rows are padded to ld = N rounded up to even.
+ * ------------------------------------------------------------------------- */
+#define SMCB_BANK_STATE 8 /* per filter: steps done t, logLt, log_mean_w of step t - 1, APF restart constant,
+                             max and sum exp of the auxiliary log-weights, resampling decided for step t (0 / 1),
+                             loglt of step t - 1 */
+
+typedef struct {
+    int32_t model, fk, scheme, tier; /* tier: SMCB_BATCH_*                                          */
+    int32_t n_params, restart;       /* restart != 0: every selected filter starts from M0 (step 0) */
+    int64_t N, T, R;                 /* particles per filter, data points, filters in the bank       */
+    int64_t t1;                      /* advance: every selected filter runs up to (excluding) step t1 */
+    const int64_t *idx;        /* (n_idx) the filters to advance, or NULL: all R; the others are not read or written */
+    int64_t n_idx;
+    double essrmin;
+    uint64_t *key;             /* (R) Philox key of each filter                                       */
+    double *params;            /* (R, n_params) model constants, layout of smcb_filter_desc.params    */
+    const double *data;        /* (T) observations, shared by every filter                            */
+    double *step_consts;       /* NULL, or (R, sc_ld) per-filter rows, or one (T) row when sc_ld == 0 */
+    int64_t sc_ld;
+    double *X;                 /* (R, 2, ld): generation s of the last two in X[r][s & 1]              */
+    double *lw;                /* (R, ld) log-weights of the last step                                 */
+    double *state;             /* (R, SMCB_BANK_STATE)                                                 */
+    int64_t *A;                /* NULL, or (R, ld): ancestors of step t1 - 1 (written only if it resampled) */
+    double *summaries;         /* NULL, or (R, T, SMCB_SUMMARY_STRIDE): rows of the steps this call runs */
+    double *cdf;               /* streaming: (scratch_rows, ld) scratch, one row per CTA of the grid   */
+    double *scratch;           /* streaming multinomial: (scratch_rows, ld + 2) exponential spacings   */
+    int64_t scratch_rows;      /* >= the grid smcb_bank_plan returns                                   */
+} smcb_bank_desc;
+
+/* out[0] = the tier, out[1] = the grid (CTAs) an advance with this descriptor takes.  Reads only the shape fields,
+ * idx and n_idx.  SMCB_ENOSYS for a combination that is not built. */
+int smcb_bank_plan(smcb_ctx *ctx, const smcb_bank_desc *desc, int64_t out[2]);
+/* SMC.__next__ (core.py:369-383) for every selected filter r from step state[r][0] (0 when restart) up to step t1;
+ * writes X, lw, state (logLt in state[r][1], loglt of step t1 - 1 in state[r][7]) and the optional A / summaries.
+ * A filter already at t1 or beyond is left as it is.  One launch, no host sync. */
+int smcb_bank_advance(smcb_ctx *ctx, const smcb_bank_desc *desc);
+/* dst[i] = src[A[i]] for i < m (X, lw, state, params, per-filter step constants, key): the outer sampler's X[A]
+ * (FancyList / all_distinct, particles/smc_samplers.py:319-361).  The first copy of an ancestor (lowest i) keeps its
+ * key; every further copy gets the key number counter + i under seed (smcb_bank_keys), so copies draw independent
+ * streams.  dst must not alias src; first: (src->R) scratch words.  Three launches, no host sync. */
+int smcb_bank_gather(smcb_ctx *ctx, const smcb_bank_desc *src, const int64_t *A, int64_t m,
+                     const smcb_bank_desc *dst, uint64_t seed, uint64_t counter, uint64_t *first);
+/* dst[i] = src[i] (all rows, key included) where accepted[i] != 0: the bank half of the Metropolis copy-where
+ * (ThetaParticles.copyto, particles/smc_samplers.py:601-611).  One launch. */
+int smcb_bank_merge(smcb_ctx *ctx, const smcb_bank_desc *dst, const smcb_bank_desc *src, const uint8_t *accepted);
+/* key[i] = the key number counter + i under seed: fmix64(fmix64(seed) + counter + i), fmix64 the splitmix64
+ * finaliser, a bijection -- distinct numbers give distinct keys.  One launch. */
+int smcb_bank_keys(smcb_ctx *ctx, uint64_t *key, int64_t n, uint64_t seed, uint64_t counter);
+/* smcb_mh_accept that also writes accepted[i] = 1 where the proposal was taken, else 0 (the mask smcb_bank_merge
+ * reads) */
+int smcb_mh_accept_flags(smcb_ctx *ctx, int64_t n, int d, double *theta, double *lprior, double *llik,
+                         double *lpost, const double *theta_p, const double *lprior_p, const double *llik_p,
+                         const double *lpost_p, const double *u_in, double *mean_acc, uint8_t *accepted);
+
 #ifdef __cplusplus
 }
 #endif

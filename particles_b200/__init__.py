@@ -16,6 +16,8 @@ def install():
     reference's model / Feynman-Kac classes stay the user-facing surface: stock models built from
     ``particles.state_space_models`` / ``particles.kalman`` are recognised by class and module name
     (``state_space_models.fused_spec``) and run on the fused kernels; their NumPy closures are never called.
+    The reference's ``particles.smc_samplers.SMC2`` of a stock 1-D model runs as ``smc_samplers.SMC2`` (its inner
+    filters in one device filter bank).
     Returns a function that restores the original binding."""
     import importlib
     import sys

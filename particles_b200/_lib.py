@@ -96,6 +96,21 @@ class BatchDesc(C.Structure):
     ]
 
 
+BANK_STATE = 8
+
+
+class BankDesc(C.Structure):
+    _fields_ = [
+        ("model", C.c_int32), ("fk", C.c_int32), ("scheme", C.c_int32), ("tier", C.c_int32),
+        ("n_params", C.c_int32), ("restart", C.c_int32),
+        ("N", C.c_int64), ("T", C.c_int64), ("R", C.c_int64), ("t1", C.c_int64),
+        ("idx", c_dp), ("n_idx", C.c_int64), ("essrmin", C.c_double),
+        ("key", c_dp), ("params", c_dp), ("data", c_dp), ("step_consts", c_dp), ("sc_ld", C.c_int64),
+        ("X", c_dp), ("lw", c_dp), ("state", c_dp), ("A", c_dp), ("summaries", c_dp),
+        ("cdf", c_dp), ("scratch", c_dp), ("scratch_rows", C.c_int64),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/smcb.h declares
 PROTOTYPES = {
     "smcb_last_error": (C.c_char_p, []),
@@ -158,6 +173,14 @@ PROTOTYPES = {
     "smcb_variance_scratch_doubles": (C.c_int64, [C.c_int64, C.c_int64, C.c_int64]),
     "smcb_batch_plan": (C.c_int, [C.c_void_p, C.POINTER(BatchDesc), C.POINTER(C.c_int64)]),
     "smcb_batch_run": (C.c_int, [C.c_void_p, C.POINTER(BatchDesc)]),
+    "smcb_bank_plan": (C.c_int, [C.c_void_p, C.POINTER(BankDesc), C.POINTER(C.c_int64)]),
+    "smcb_bank_advance": (C.c_int, [C.c_void_p, C.POINTER(BankDesc)]),
+    "smcb_bank_gather": (C.c_int, [C.c_void_p, C.POINTER(BankDesc), c_dp, C.c_int64, C.POINTER(BankDesc),
+                                   C.c_uint64, C.c_uint64, c_dp]),
+    "smcb_bank_merge": (C.c_int, [C.c_void_p, C.POINTER(BankDesc), C.POINTER(BankDesc), c_dp]),
+    "smcb_bank_keys": (C.c_int, [C.c_void_p, c_dp, C.c_int64, C.c_uint64, C.c_uint64]),
+    "smcb_mh_accept_flags": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
+                                       c_dp, c_dp, c_dp, c_dp]),
 }
 
 _lib = None

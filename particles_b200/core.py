@@ -306,6 +306,8 @@ class SMC:
                  noise=None):
         require_cuda()
         _lib.load()
+        from .smc_samplers import from_reference_smc2
+        fk = from_reference_smc2(fk) or fk          # the reference's SMC2 of a stock 1-D model: the filter bank
         if qmc:
             raise NotImplementedError("SQMC (qmc=True) is outside the accelerated path")
         if resampling not in rs.rs_funcs:

@@ -139,7 +139,8 @@ __global__ void __launch_bounds__(kSampBlock) k_mh_accept(int64_t n, int d, doub
                                                          const double *__restrict__ lpost_p,
                                                          Philox key, uint64_t call,
                                                          const double *__restrict__ u_in, double *partials,
-                                                         unsigned int *ticket, double *mean_acc) {
+                                                         unsigned int *ticket, double *mean_acc,
+                                                         uint8_t *accepted) {
     __shared__ double s_red[kSampBlock / 32];
     __shared__ bool s_last;
     const int64_t i = (int64_t)blockIdx.x * kSampBlock + threadIdx.x;
@@ -158,6 +159,7 @@ __global__ void __launch_bounds__(kSampBlock) k_mh_accept(int64_t n, int d, doub
             for (int j = 0; j < d; j++) theta[i * d + j] = theta_p[i * d + j];
             lprior[i] = lprior_p[i]; llik[i] = llik_p[i]; lpost[i] = lpost_p[i];
         }
+        if (accepted) accepted[i] = (u < pb) ? 1 : 0;
     }
     double acc = pb;
 #pragma unroll
@@ -393,11 +395,11 @@ extern "C" int smcb_rw_propose(smcb_ctx *c, const double *theta, int64_t n, int 
     return SMCB_OK;
 }
 
-// ArrayMetropolis.step accept / copyto (smc_samplers.py:605-611); mean_acc: device scalar
-extern "C" int smcb_mh_accept(smcb_ctx *c, int64_t n, int d, double *theta, double *lprior, double *llik,
-                              double *lpost, const double *theta_p, const double *lprior_p,
-                              const double *llik_p, const double *lpost_p, const double *u_in,
-                              double *mean_acc) {
+// ArrayMetropolis.step accept / copyto (smc_samplers.py:605-611); mean_acc: device scalar; accepted: NULL or (n)
+extern "C" int smcb_mh_accept_flags(smcb_ctx *c, int64_t n, int d, double *theta, double *lprior, double *llik,
+                                    double *lpost, const double *theta_p, const double *lprior_p,
+                                    const double *llik_p, const double *lpost_p, const double *u_in,
+                                    double *mean_acc, uint8_t *accepted) {
     SMCB_REQUIRE(c && theta && lprior && llik && lpost && theta_p && lprior_p && llik_p && lpost_p && mean_acc,
                  "smcb_mh_accept: NULL argument");
     SMCB_REQUIRE(n >= 1 && d >= 1, "smcb_mh_accept: bad sizes");
@@ -405,8 +407,16 @@ extern "C" int smcb_mh_accept(smcb_ctx *c, int64_t n, int d, double *theta, doub
     SMCB_REQUIRE((size_t)grid <= kWsPartials, "smcb_mh_accept: too many particles for the workspace");
     const uint64_t call = u_in ? 0 : c->api_counter++;
     LAUNCHK(c, k_mh_accept, grid, kSampBlock, 0, n, d, theta, lprior, llik, lpost, theta_p, lprior_p, llik_p,
-            lpost_p, key_of(c->seed), call, u_in, c->ws, c->counters + 2, mean_acc);
+            lpost_p, key_of(c->seed), call, u_in, c->ws, c->counters + 2, mean_acc, accepted);
     return SMCB_OK;
+}
+
+extern "C" int smcb_mh_accept(smcb_ctx *c, int64_t n, int d, double *theta, double *lprior, double *llik,
+                              double *lpost, const double *theta_p, const double *lprior_p,
+                              const double *llik_p, const double *lpost_p, const double *u_in,
+                              double *mean_acc) {
+    return smcb_mh_accept_flags(c, n, d, theta, lprior, llik, lpost, theta_p, lprior_p, llik_p, lpost_p, u_in,
+                                mean_acc, nullptr);
 }
 
 // ---------------------------------------------------------------------------

@@ -189,6 +189,86 @@ class Logistic(LocScaleDist, _Univariate):
         return (la if la is not None else l0) + (sa if sa is not None else s0) * (torch.log(u) - torch.log1p(-u))
 
 
+def _host(v):
+    """A log-density or draw (CUDA tensor, NumPy array or scalar) as a host fp64 array."""
+    if isinstance(v, torch.Tensor):
+        return v.detach().cpu().numpy().astype(np.float64)
+    return np.asarray(v, dtype=np.float64)
+
+
+class Uniform(ProbDist):
+    """Uniform([a, b]) -- particles/distributions.py:399-414.  A law of static parameters: ``logpdf`` runs on the
+    host (NumPy in, NumPy out, scipy.stats.uniform's closed support); ``rvs`` draws from the context's Philox
+    stream."""
+
+    def __init__(self, a=0.0, b=1.0):
+        self.a, self.b = a, b
+        self.scale = b - a
+
+    def rvs(self, size=None):
+        n = 1 if size is None else int(size)
+        ctx = context()
+        u = empty(n)
+        _lib.check(ctx.lib.smcb_uniform(ctx.handle, ptr(u), n))
+        return self.a + self.scale * u
+
+    def logpdf(self, x):
+        x = _host(x)
+        return np.where((x >= self.a) & (x <= self.a + self.scale), -np.log(self.scale), -np.inf)
+
+
+class Beta(ProbDist):
+    """Beta(a, b) -- particles/distributions.py:319-333; ``logpdf`` on the host (scipy.stats.beta's formula),
+    ``rvs`` from torch's generator as Gamma.rvs."""
+
+    def __init__(self, a=1.0, b=1.0):
+        self.a, self.b = a, b
+
+    def rvs(self, size=None):
+        n = 1 if size is None else int(size)
+        a = torch.full((n,), float(self.a), dtype=torch.float64, device="cuda")
+        return torch.distributions.Beta(a, torch.full_like(a, float(self.b))).sample()
+
+    def logpdf(self, x):
+        from scipy.special import betaln, xlog1py, xlogy
+        x = _host(x)
+        a, b = float(self.a), float(self.b)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            lp = xlog1py(b - 1.0, -x) + xlogy(a - 1.0, x) - betaln(a, b)
+        return np.where((x > 0.0) & (x < 1.0), lp, -np.inf)
+
+
+class StructDist(ProbDist):
+    """Independent laws of named scalar parameters -- particles/distributions.py:1149-1214.  ``rvs(size)`` returns a
+    NumPy structured array (fields in sorted order for a dict, as in the reference), ``logpdf(theta)`` the host
+    array of the summed log-densities.  The component laws may be this package's (device draws, copied to the host)
+    or any object with the same two methods; a callable law (``Cond``) receives the structured array."""
+
+    def __init__(self, laws):
+        from collections import OrderedDict
+        if isinstance(laws, OrderedDict):
+            self.laws = laws
+        elif isinstance(laws, dict):
+            self.laws = OrderedDict([(k, laws[k]) for k in sorted(laws)])
+        else:
+            raise TypeError("recdist class requires a dict or an ordered dict to be instantiated")
+        self.dtype = [(k, float) for k in self.laws]
+
+    def logpdf(self, theta):
+        lp = 0.0
+        for par, law in self.laws.items():
+            cond = law(theta) if callable(law) else law
+            lp = lp + _host(cond.logpdf(theta[par]))
+        return lp
+
+    def rvs(self, size=1):
+        out = np.empty(size, dtype=self.dtype)
+        for par, law in self.laws.items():
+            cond = law(out) if callable(law) else law
+            out[par] = _host(cond.rvs(size=size)).reshape(-1)
+        return out
+
+
 class Categorical(ProbDist):
     """Categorical(p), p (k,) or (N, k) -- particles/distributions.py:598-628."""
     dtype = np.int64

@@ -312,3 +312,272 @@ class AdaptiveTempering(Tempering):
     def M(self, t, xp):
         xp.shared["rs_flag"] = True
         return self._M(t, xp, xp.shared["exponents"][-1])
+
+
+# ---------------------------------------------------------------------------------------------------------- SMC^2
+def _as_struct(arr, names):
+    """(n, p) host array -> structured array with one float field per column."""
+    out = np.empty(arr.shape[0], dtype=[(k, float) for k in names])
+    for i, k in enumerate(names):
+        out[k] = arr[:, i]
+    return out
+
+
+class SMC2Particles(ThetaParticles):
+    """The particles of ``SMC2``: ``theta_dev`` (n, p) fp64 CUDA tensor of the parameters (columns ``names``, the
+    prior's fields), ``lprior``, ``llik`` (each filter's logLt), ``lpost`` (n,) and ``bank``, the n inner filters
+    (``bank.FilterBank``) in place of the reference's list ``pfs``.  ``theta`` is the NumPy structured array of the
+    reference's particles, materialised from the device on each access (``X.theta['sigma']``).  Indexing by an
+    int64 tensor gathers the fields and the bank; the bank copies of a repeated ancestor after the first draw new keys
+    from the sampler's key counter ``keys``."""
+
+    _META = ("shared", "names", "bank", "keys")
+
+    def __init__(self, shared=None, names=(), bank=None, keys=None, **fields):
+        super().__init__(shared=shared, **fields)
+        self.names, self.bank, self.keys = tuple(names), bank, keys
+
+    @property
+    def dict_fields(self):
+        return {k: v for k, v in self.__dict__.items() if k not in self._META}
+
+    @property
+    def theta(self):
+        return _as_struct(self.theta_dev.cpu().numpy(), self.names)
+
+    @property
+    def Nx(self):
+        return self.bank.N
+
+    def _like(self, fields, bank):
+        return self.__class__(shared=self.shared.copy(), names=self.names, bank=bank, keys=self.keys, **fields)
+
+    def __getitem__(self, key):
+        if not (isinstance(key, torch.Tensor) and key.dtype == torch.int64):
+            key = torch.as_tensor(np.arange(self.N)[key], dtype=torch.int64, device=self.theta_dev.device)
+        x = ThetaParticles.__getitem__(ThetaParticles(**self.dict_fields), key)
+        bank = self.bank.gather(key, self.keys.seed, self.keys.take(key.shape[0]))
+        return self._like(x.dict_fields, bank)
+
+    def copy(self):
+        """A copy whose filters continue independently of the originals (the reference deep-copies its filters, whose
+        futures then draw different numbers from the global stream): the rows are copied, the keys are fresh."""
+        b = self.bank.empty_like()
+        for name in ("X", "lw", "state", "params") + (("sc",) if b.sc is not None else ()):
+            getattr(b, name).copy_(getattr(self.bank, name))
+        b.fresh_keys(self.keys.seed, self.keys.take(b.R))
+        b.timer = self.bank.timer
+        return self._like({k: v.clone() for k, v in self.dict_fields.items()}, b)
+
+    @classmethod
+    def concatenate(cls, *xs):
+        from .bank import FilterBank
+        fields = {k: torch.cat([getattr(x, k) for x in xs]) for k in xs[0].dict_fields}
+        return xs[0]._like(fields, FilterBank.concatenate(*[x.bank for x in xs]))
+
+
+class _KeyCounter:
+    """The sampler's seed and the number of inner-filter keys drawn so far: key number c is
+    fmix64(fmix64(seed) + c) (smcb_bank_keys), so no two filters of a run ever share a key."""
+
+    def __init__(self, seed):
+        self.seed, self.count = int(seed) & (2 ** 64 - 1), 0
+
+    def take(self, n):
+        c = self.count
+        self.count += int(n)
+        return c
+
+
+class BankRandomWalk(ArrayRandomWalk):
+    """Gaussian random-walk Metropolis on ``theta_dev`` whose target re-runs the proposals' filters: the accepted
+    proposals' filters replace the current ones (smcb_mh_accept_flags + smcb_bank_merge)."""
+
+    def calibrate(self, W, x):
+        n, d = x.theta_dev.shape
+        ctx = context()
+        L = empty(d * d).reshape(d, d)
+        _lib.check(ctx.lib.smcb_rw_calibrate(ctx.handle, ptr(as_device(W)), ptr(x.theta_dev), n, d,
+                                             2.38 / np.sqrt(d), ptr(L)))
+        x.shared["chol_cov"] = L
+
+    def step(self, x, target):
+        ctx = context()
+        n, d = x.theta_dev.shape
+        xprop = x._like({"theta_dev": torch.empty_like(x.theta_dev)}, None)
+        _lib.check(ctx.lib.smcb_rw_propose(ctx.handle, ptr(x.theta_dev), n, d, ptr(x.shared["chol_cov"]), None,
+                                           ptr(xprop.theta_dev)))
+        target(xprop)
+        acc = empty(1)
+        flags = torch.empty(n, dtype=torch.uint8, device=x.theta_dev.device)
+        _lib.check(ctx.lib.smcb_mh_accept_flags(
+            ctx.handle, n, d, ptr(x.theta_dev), ptr(x.lprior), ptr(x.llik), ptr(x.lpost), ptr(xprop.theta_dev),
+            ptr(xprop.lprior), ptr(xprop.llik), ptr(xprop.lpost), None, ptr(acc), ptr(flags)))
+        x.bank.merge(xprop.bank, flags)
+        return acc
+
+
+class SMC2(FKSMCsampler):
+    """SMC^2 (smc_samplers.py:1038-1167): an SMC sampler over theta whose likelihood factors are estimated by one
+    particle filter per theta-particle.  Same constructor as the reference; the inner filters are one
+    ``bank.FilterBank`` on the device, advanced one step for every theta-particle in ONE launch per SMC^2 step, and
+    re-run from step 0 for all proposals of an MCMC step (or all particles of an exchange step) in one launch.
+
+    ``ssm_cls`` must be one of the stock 1-D models (``bank.SUPPORTED``), of this package or the reference;
+    ``fk_cls`` one of the stock Feynman-Kac kinds (Bootstrap by default).  ``smc_options`` passes ``resampling``
+    and ``ESSrmin`` to the inner filters (``qmc=True`` is not built).  ``prior`` is duck-typed: ``rvs(size)`` returns a
+    structured array of scalar fields, ``logpdf(theta)`` their joint log-density, evaluated on the host
+    (``distributions.StructDist``, or the reference's own).  ``seed``: the key of the inner filters' streams;
+    by default it is drawn from the device generator when the sampler starts, so ``SMC(seed=s)`` fixes it."""
+
+    def __init__(self, ssm_cls=None, prior=None, data=None, smc_options=None, fk_cls=None, init_Nx=100,
+                 ar_to_increase_Nx=-1.0, wastefree=True, len_chain=10, move=None, seed=None, tier="auto"):
+        if move is None:
+            seq = MCMCSequenceWF if wastefree else AdaptiveMCMCSequence
+            move = seq(mcmc=BankRandomWalk(), len_chain=len_chain)
+        super().__init__(model=None, wastefree=wastefree, len_chain=len_chain, move=move)
+        self.smc_options = {"collect": "off"}
+        if smc_options is not None:
+            self.smc_options.update(smc_options)
+        if "model" in self.smc_options or "data" in self.smc_options:
+            raise ValueError("SMC2: options model and data are not allowed in smc_options")
+        if self.smc_options.get("qmc"):
+            raise NotImplementedError("SMC2 over SQMC inner filters (qmc=True) is not built")
+        self.resampling = self.smc_options.get("resampling", "systematic")
+        if self.resampling not in _lib.FUSED_SCHEMES:
+            raise NotImplementedError("SMC2: the inner filters resample with one of %s" % (_lib.FUSED_SCHEMES,))
+        self.ESSrmin_inner = float(self.smc_options.get("ESSrmin", 0.5))
+        from .state_space_models import _FK_KINDS, Bootstrap
+        self.fk_cls = Bootstrap if fk_cls is None else fk_cls
+        self.fk_kind = dict(_FK_KINDS).get(getattr(self.fk_cls, "__name__", None))
+        self.ssm_cls, self.prior, self.data = ssm_cls, prior, data
+        self.init_Nx, self.ar_to_increase_Nx = int(init_Nx), ar_to_increase_Nx
+        self.seed, self.tier = seed, tier
+        self._map = None
+        if data is not None:
+            self._setup()
+
+    def _setup(self):
+        from .bank import ThetaMap
+        from .state_space_models import _flat_data
+        flat = _flat_data(self.data, 1).reshape(-1)
+        names = list(getattr(self.prior, "laws", {}).keys()) or list(self.prior.rvs(size=1).dtype.names)
+        self._map = ThetaMap(self.ssm_cls, names, flat)
+        if self.fk_kind is None or (self.fk_kind != _lib.FK_BOOTSTRAP and not self._map.proposal) or (
+                self.fk_kind == _lib.FK_GUIDED and self._map.name == "ThetaLogistic"):
+            raise NotImplementedError("SMC2: Feynman-Kac class %r is not built for %s on the device"
+                                      % (self.fk_cls, self._map.name))
+        self._data_dev = self._sc_dev = None      # uploaded with the first bank
+        self.timer = None          # None, or a list that receives the CUDA events of every bank launch
+
+    @property
+    def T(self):
+        return 0 if self.data is None else len(self.data)
+
+    # ------------------------------------------------------------------ theta -> filters
+    def _bank(self, theta_dev, Nx, keys):
+        from .bank import FilterBank
+        m = self._map
+        n = theta_dev.shape[0]
+        if self._data_dev is None:
+            self._data_dev = as_device(m.data)
+            self._sc_dev = None if m.shared_sc is None else as_device(m.shared_sc)
+        b = FilterBank(m.model, self.fk_kind, self.resampling, Nx, n, self._data_dev, m.n_params, self.ESSrmin_inner,
+                       shared_sc=self._sc_dev, per_filter_sc=m.name == "Gordon_etal", tier=self.tier)
+        th = theta_dev.cpu().numpy()
+        b.set_rows(m.params(th), m.step_consts(th))
+        b.fresh_keys(keys.seed, keys.take(n))
+        b.timer = self.timer
+        return b
+
+    def current_target(self, t, Nx):
+        """smc_samplers.py:1129-1143: new filters for every particle, prior, and -- for t >= 0 -- the filters of the
+        particles with a finite prior re-run over steps 0..t in one launch; lpost = lprior + logLt."""
+        def func(x):
+            x.bank = self._bank(x.theta_dev, Nx, x.keys)
+            lp = np.asarray(self.prior.logpdf(x.theta), dtype=np.float64)
+            lp = np.array(np.broadcast_to(lp, (x.theta_dev.shape[0],)))
+            x.lprior = as_device(lp)
+            if t >= 0:
+                idx = np.flatnonzero(np.isfinite(lp))
+                if idx.size:
+                    x.bank.advance(t + 1, idx=as_device(idx, dtype=torch.int64), restart=True)
+            x.llik = x.bank.logLt.clone()
+            x.lpost = x.lprior + x.llik
+        return func
+
+    def _M0(self, N):
+        if self._map is None:
+            self._setup()
+        seed = self.seed
+        if seed is None:                       # from the device generator: SMC(seed=s) fixes the inner keys
+            ctx = context()
+            u = empty(2)
+            _lib.check(ctx.lib.smcb_uniform(ctx.handle, ptr(u), 2))
+            hi, lo = (int(v * 2.0 ** 32) for v in u.cpu().numpy())
+            seed = (hi << 32) | lo
+        th = self.prior.rvs(size=N)
+        names = self._map.names = list(th.dtype.names)
+        cols = np.stack([np.asarray(th[k], dtype=np.float64).reshape(N) for k in names], axis=1)
+        x0 = SMC2Particles(shared={"Nxs": [self.init_Nx]}, names=names, keys=_KeyCounter(seed),
+                           theta_dev=as_device(cols))
+        self.current_target(-1, self.init_Nx)(x0)
+        return x0
+
+    def logG(self, t, xp, x):
+        """smc_samplers.py:1099-1120: exchange step if the last move accepted too little, then every filter advances
+        by step t (one launch); the increments loglt are the log-weights."""
+        we_increase_Nx = False
+        if x.shared.get("rs_flag", False) and x.shared.get("acc_rates"):
+            ars = x.shared["acc_rates"][-1]          # the last move's list of mean acceptance rates (device scalars)
+            ar = float(torch.cat([a.reshape(1) for a in ars]).mean())
+            we_increase_Nx = ar < self.ar_to_increase_Nx
+        liw_Nx = None
+        if we_increase_Nx:
+            liw_Nx = self.exchange_step(x, t, 2 * x.bank.N)
+        x.bank.advance(t + 1)
+        lpyt = x.bank.loglt.clone()
+        x.lpost = x.lpost + lpyt
+        x.llik = x.bank.logLt.clone()
+        if t > 0:
+            x.shared["Nxs"].append(x.bank.N)
+        return lpyt + liw_Nx if we_increase_Nx else lpyt
+
+    def M(self, t, xp):
+        if xp.shared["rs_flag"]:
+            return self.move(xp, self.current_target(t - 1, xp.bank.N))
+        return xp
+
+    def exchange_step(self, x, t, new_Nx):
+        """smc_samplers.py:1159-1163: every filter re-run over steps 0..t-1 at new_Nx particles."""
+        old_lpost = x.lpost.clone()
+        self.current_target(t - 1, new_Nx)(x)
+        return x.lpost - old_lpost
+
+    def default_moments(self, W, x):
+        """Weighted mean and variance of every parameter, as structured arrays (the reference's
+        wmean_and_var_str_array)."""
+        m = rs.wmean_and_var(W, x.theta_dev)
+        mean, var = np.atleast_1d(m["mean"]), np.atleast_1d(m["var"])
+        return {"mean": _as_struct(mean[None, :], x.names), "var": _as_struct(var[None, :], x.names)}
+
+    def summary_format(self, smc):
+        return super().summary_format(smc) + ", Nx=%i" % smc.X.bank.N
+
+
+def from_reference_smc2(fk):
+    """``SMC2`` for the reference's own ``particles.smc_samplers.SMC2`` object when its ``ssm_cls`` is a stock 1-D
+    model (recognised by class name and module, as ``state_space_models.fused_spec`` does), else None: that object
+    then keeps its own path.  The sampler takes the reference object's model, prior, data, options, Feynman-Kac
+    class, Nx schedule and chain length; the move is this package's (random walk over the filter bank)."""
+    cls = type(fk)
+    if cls.__name__ != "SMC2" or cls.__module__ != "particles.smc_samplers":
+        return None
+    move = getattr(fk, "move", None)
+    len_chain = getattr(move, "nsteps", getattr(fk, "len_chain", 10) - 1) + 1
+    try:
+        return SMC2(ssm_cls=fk.ssm_cls, prior=fk.prior, data=fk.data, smc_options=dict(fk.smc_options),
+                    fk_cls=fk.fk_cls, init_Nx=fk.init_Nx, ar_to_increase_Nx=fk.ar_to_increase_Nx,
+                    wastefree=fk.wastefree, len_chain=len_chain)
+    except NotImplementedError:
+        return None
