@@ -501,6 +501,47 @@ int smcb_mh_accept_flags(smcb_ctx *ctx, int64_t n, int d, double *theta, double 
                          double *lpost, const double *theta_p, const double *lprior_p, const double *llik_p,
                          const double *lpost_p, const double *u_in, double *mean_acc, uint8_t *accepted);
 
+/* ---------------------------------------------------------------------------
+ * conditional SMC (Particle Gibbs, particles/mcmc.py:453-475 and 594-609): R chains, one filter of N particles each,
+ * of one 1-D model and the Bootstrap or Guided kind, multinomial resampling when ESS < ESSrmin N, each with its own
+ * model constants, Philox key and reference path x* (csrc/smcb_pmcmc.cu).  Slot 0 is pinned to x*: x*[0] at step 0,
+ * then ancestor 0 and state x*[t], weighted by logG(t, x*[t-1], x*[t]).  With pin = 0 the same pass runs
+ * unconditionally and chain r gives the bits of the filter bank's multinomial filter with key[r].  The whole history
+ * is kept, and the same launch draws one new trajectory per chain from it.  Rows are padded to ld = N rounded up to
+ * even.
+ * ------------------------------------------------------------------------- */
+#define SMCB_CSMC_GENEALOGY 0 /* trace the ancestors of one draw from W_{T-1} (smoothing.py:256-269)     */
+#define SMCB_CSMC_BACKWARD 1  /* one backward draw per step, backward_sampling_ON2(1) (smoothing.py:291-311) */
+
+typedef struct {
+    int32_t model, fk, n_params, draw; /* fk: SMCB_FK_BOOTSTRAP or SMCB_FK_GUIDED; draw: SMCB_CSMC_*     */
+    int32_t pin, reserved0;            /* pin != 0: slot 0 follows xstar                                 */
+    int64_t N, T, R;                   /* particles per chain, data points, chains                      */
+    double essrmin;
+    const uint64_t *key;       /* (R) Philox key of each chain                                         */
+    const double *params;      /* (R, n_params) model constants, layout of smcb_filter_desc.params     */
+    const double *data;        /* (R, data_ld) observations; data_ld = 0: one (T) row shared by all    */
+    int64_t data_ld;
+    const double *step_consts; /* NULL, or (R, sc_ld) per-chain rows, or one (T) row when sc_ld == 0   */
+    int64_t sc_ld;
+    const double *xstar;       /* (R, T) reference paths (read only when pin != 0)                     */
+    double *X;                 /* (R, T, ld) particles of every step                                   */
+    double *lw;                /* (R, T, ld) log-weights of every step                                 */
+    int64_t *A;                /* (R, T, ld) ancestors of every step (arange where a step does not resample) */
+    double *traj;              /* (R, T) the drawn trajectory                                          */
+    double *logLt;             /* (R) log-likelihood estimate                                          */
+    double *summaries;         /* NULL, or (R, T, SMCB_SUMMARY_STRIDE)                                 */
+    const double *z_in;        /* NULL, or (R, T, N) injected normals                                  */
+    const double *u_in;        /* NULL, or (R, T, N + 1) injected uniforms of the multinomial spacings */
+    const double *ud_in;       /* NULL, or (R, T) injected uniforms of the trajectory draw at step t   */
+} smcb_csmc_desc;
+
+/* out[0] = the largest N the shared memory of this device holds for this model and kind, out[1] = the grid (CTAs).
+ * SMCB_ENOSYS for a combination that is not built or an N above the bound. */
+int smcb_csmc_plan(smcb_ctx *ctx, const smcb_csmc_desc *desc, int64_t out[2]);
+/* the forward pass and the trajectory draw of every chain: one launch on the context's stream, no host sync */
+int smcb_csmc_run(smcb_ctx *ctx, const smcb_csmc_desc *desc);
+
 #ifdef __cplusplus
 }
 #endif

@@ -111,6 +111,21 @@ class BankDesc(C.Structure):
     ]
 
 
+CSMC_GENEALOGY, CSMC_BACKWARD = 0, 1
+
+
+class CsmcDesc(C.Structure):
+    _fields_ = [
+        ("model", C.c_int32), ("fk", C.c_int32), ("n_params", C.c_int32), ("draw", C.c_int32),
+        ("pin", C.c_int32), ("reserved0", C.c_int32),
+        ("N", C.c_int64), ("T", C.c_int64), ("R", C.c_int64), ("essrmin", C.c_double),
+        ("key", c_dp), ("params", c_dp), ("data", c_dp), ("data_ld", C.c_int64),
+        ("step_consts", c_dp), ("sc_ld", C.c_int64), ("xstar", c_dp),
+        ("X", c_dp), ("lw", c_dp), ("A", c_dp), ("traj", c_dp), ("logLt", c_dp), ("summaries", c_dp),
+        ("z_in", c_dp), ("u_in", c_dp), ("ud_in", c_dp),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/smcb.h declares
 PROTOTYPES = {
     "smcb_last_error": (C.c_char_p, []),
@@ -181,6 +196,8 @@ PROTOTYPES = {
     "smcb_bank_keys": (C.c_int, [C.c_void_p, c_dp, C.c_int64, C.c_uint64, C.c_uint64]),
     "smcb_mh_accept_flags": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                        c_dp, c_dp, c_dp, c_dp]),
+    "smcb_csmc_plan": (C.c_int, [C.c_void_p, C.POINTER(CsmcDesc), C.POINTER(C.c_int64)]),
+    "smcb_csmc_run": (C.c_int, [C.c_void_p, C.POINTER(CsmcDesc)]),
 }
 
 _lib = None

@@ -289,6 +289,31 @@ __device__ __forceinline__ void fk_move(const M &m, const StepK &k, double xp, d
     }
 }
 
+// logG(0, None, x) at a given state x: the delta of fk_init, for a particle that is not drawn (the pinned path of the
+// conditional filter, smcb_pmcmc.cu)
+template <class M, int FK>
+__device__ __forceinline__ double fk_logG0(const M &m, const StepK &k, double x) {
+    if (FkTraits<FK>::guided) {
+        double loc, scale, ls, l0, s0, ls0;
+        m.prop0(k, loc, scale, ls);
+        m.init(l0, s0, ls0);
+        return normal_logpdf_ls(x, l0, s0, ls0) + m.obs_logpdf(k, x, x) - normal_logpdf_ls(x, loc, scale, ls);
+    }
+    return m.obs_logpdf(k, x, x);
+}
+
+// logG(t, xp, x) at given states xp, x: the delta of fk_move
+template <class M, int FK>
+__device__ __forceinline__ double fk_logG(const M &m, const StepK &k, double xp, double x) {
+    if (FkTraits<FK>::guided) {
+        double loc, scale, ls, lt, st, lst;
+        m.prop(k, xp, loc, scale, ls);
+        m.trans(k, xp, lt, st, lst);
+        return normal_logpdf_ls(x, lt, st, lst) + m.obs_logpdf(k, xp, x) - normal_logpdf_ls(x, loc, scale, ls);
+    }
+    return m.obs_logpdf(k, xp, x);
+}
+
 // ---------------------------------------------------------------------------
 // d-dimensional models (SoA state): small dense algebra in registers, no tensor cores
 // (SURVEY.md section 7 step 7: a 4x4 triangular matvec is 10 FMAs).
