@@ -168,6 +168,14 @@ int smcb_logistic_wf_move(smcb_ctx *ctx, int64_t M, int d, int P, const double *
                           double *theta_out, double *lprior_out, double *llik_out, double *lpost_out,
                           double *pb_out);
 
+/* IBIS.logG, smc_samplers.py:773-776, for the logistic-regression model: logpyt of the data rows [r0, r0 + K) of
+ * data (n_data, d) for n particles, added one row at a time in row order (a NaN log-weight becomes -inf after each
+ * row).  commit != 0: lw, lpost and llik += every row, in place (lpost / llik may be NULL); commit == 0:
+ * scratch (K, n) row k = lw + the rows r0 .. r0 + k, and nothing else is written.  Same per-row bits as a one-row
+ * smcb_logistic_target. */
+int smcb_logistic_logpyt(smcb_ctx *ctx, const double *theta, int64_t n, int d, const double *data, int64_t n_data,
+                         int64_t r0, int64_t K, int commit, double *lw, double *lpost, double *llik, double *scratch);
+
 /* AdaptiveTempering's control plane on the device (no host round trip inside a tempering step):
  * next_annealing_epn, smc_samplers.py:876-895: the exponent at which ESS(delta * llik) = alpha * n, by an 11-pass
  * 16-way bracketing search whose state stays in device memory; out_dev[0] = new exponent (1.0 if the whole step fits) */

@@ -589,12 +589,83 @@ class SMC:
                     self.summaries._extend_moments(self._engine.mom.cpu().numpy()[first:T], self._engine.dim)
                 for col in online:
                     col._flush()
+        elif self._ibis_stretches():
+            self._run_ibis()
         else:
             for _ in self:
                 pass
             if self.fused:
                 torch.cuda.synchronize()
         self.cpu_time = time.perf_counter() - t0
+
+    # ------------------------------------------------------- IBIS stretches
+    def _ibis_stretches(self):
+        """True for an IBIS run over a model with a device likelihood, without verbose output, history or
+        collectors beyond the defaults, whose resampling rule is FKSMCsampler's: ``run()`` may then add the data
+        rows of a stretch of non-resampling steps with one host read."""
+        from .smc_samplers import IBIS, FKSMCsampler
+        fk = self.fk
+        return (isinstance(fk, IBIS) and hasattr(fk.model, "logpyt_rows") and not self.verbose and not self.hist
+                and (self.summaries is None or self.summaries.only_defaults)
+                and type(fk).time_to_resample is FKSMCsampler.time_to_resample
+                and type(fk).done is FeynmanKac.done and not _is_apf(fk))
+
+    def _run_ibis(self):
+        """The per-step loop, with every run of non-resampling steps done as stretches (DESIGN.md section 5.10).
+        From the state after step t - 1 whose ESS stays above the threshold, the rows t .. t + K - 1 are scanned
+        into a (K, n) scratch buffer of cumulative log-weights, each scratch row is normalised into a (K, 4) table
+        (smcb_normalise: the bits the per-step path computes), the table is read once, and the rows up to the first
+        one whose ESS falls below ESSrmin * X.N are committed.  The resampling step that follows, and the steps
+        whose predecessor is below the threshold, run through the iterator.  Same bits as ``for _ in pf: pass``."""
+        fk, p, ctx = self.fk, self._p, context()
+        st = self._ibis_stats = {"stretches": 0, "rows": 0, "reads": 0, "scanned": 0, "last": 0}
+        K = IBIS_K0
+        while not fk.done(self):
+            X = p["X"]
+            if self.t == 0 or p["wgts"].ESS < X.N * self.ESSrmin:      # step t resamples (time_to_resample)
+                next(self)
+                K = IBIS_K0
+                continue
+            n, t = X.N, self.t
+            k = max(1, min(K, IBIS_SCRATCH_BYTES // (8 * n), fk.T - t))
+            scratch, table = empty((k, n)), empty((k, 4))
+            lw = p["wgts"].lw
+            fk.model.logpyt_rows(X.theta, t, k, lw, scratch=scratch)
+            for r in range(k):
+                _lib.check(ctx.lib.smcb_normalise(ctx.handle, ptr(scratch[r]), n, None, ptr(table[r])))
+            tab = table.cpu().numpy()                     # the one device->host read of the stretch
+            below = np.flatnonzero(tab[:, 2] < n * self.ESSrmin)
+            m = int(below[0]) + 1 if below.size else k
+            fk.model.logpyt_rows(X.theta, t, m, lw, X.lpost, X.llik)
+            st["stretches"] += 1
+            st["reads"] += 1
+            st["rows"] += m
+            st["scanned"] += k
+            st["last"] = t + m
+            wgts = rs.Weights._from_device_stats(lw, table[m - 1])
+            wgts._host = tab[m - 1]
+            ess, logLts = [], []
+            for r in range(m):                            # compute_summaries, step by step
+                prec, p["log_mean_w"] = p["log_mean_w"], float(tab[r, 1])
+                p["loglt"] = p["log_mean_w"] - prec
+                p["logLt"] += p["loglt"]
+                ess.append(float(tab[r, 2]))
+                logLts.append(p["logLt"])
+            p["wgts"] = p["aux"] = wgts
+            p["rs_flag"] = X.shared["rs_flag"] = False
+            p["A"] = torch.arange(self.N, device="cuda")
+            p["Xp"] = X
+            if self.summaries:
+                self.summaries._extend_defaults(ess, logLts, [False] * m)
+            self.t += m
+            self._done = self.t
+            K = K if below.size else K * IBIS_K_GROWTH
+
+
+# IBIS stretches (SMC._run_ibis): the first stretch after a resampling scans IBIS_K0 rows, each stretch that ends
+# without an ESS crossing multiplies the next one's rows by IBIS_K_GROWTH, and the (K, n) fp64 scratch buffer stays
+# within IBIS_SCRATCH_BYTES.  Chosen by measurement with tools/bench_ibis.py (DESIGN.md section 5.10).
+IBIS_K0, IBIS_K_GROWTH, IBIS_SCRATCH_BYTES = 8, 2, 64 << 20
 
 
 # ---------------------------------------------------------------------------------------------------- multiSMC

@@ -710,3 +710,111 @@ extern "C" int smcb_essl_grid(smcb_ctx *c, const double *lw, int64_t n, double l
     LAUNCHK(c, k_ctl_root_pass, grid, kCtlBlock, 0, lw, n, 0.0, state, partials, c->counters + 9, 0, out32_dev);
     return SMCB_OK;
 }
+
+// ---------------------------------------------------------------------------
+// IBIS reweighting (IBIS.logG, smc_samplers.py:773-776, for the logistic model): the log-likelihood of the data rows
+// [r0, r0 + K) for n particles, added to the log-weights ONE ROW AT A TIME, in row order.
+//   scan   (COMMIT = false): scratch[k * n + i] = lw[i] + sum_{r <= k} logpyt_r(theta_i); lw is not written.
+//   commit (COMMIT = true):  lw[i], lpost[i] and llik[i] += logpyt_r(theta_i) for r = r0 .. r0 + K - 1, in place
+//                            (lpost / llik may be NULL).
+// A NaN log-weight becomes -inf after each row, as smcb_normalise rewrites it after each step of the per-step path,
+// so scratch row k and a commit through row k hold the bits of k + 1 single-row steps.  The dot product and
+// neg_softplus_neg are those of k_logistic_target (theta in registers, two particles per thread, rows staged in
+// shared memory, fma over the padded coordinates in order): a one-row logpyt has the bits of a one-row target.
+// ---------------------------------------------------------------------------
+namespace smcb {
+
+template <int D, bool COMMIT>
+__global__ void __launch_bounds__(kSampBlock) k_logistic_logpyt(
+    const double *__restrict__ theta, int64_t n, int d, const double *__restrict__ data, int64_t r0, int64_t K,
+    double *__restrict__ lw, double *__restrict__ lpost, double *__restrict__ llik, double *__restrict__ scratch) {
+    __shared__ __align__(16) double s_x[kRowsPerTile * D];
+    const int64_t i0 = 2 * ((int64_t)blockIdx.x * kSampBlock + threadIdx.x);
+    const bool v0 = i0 < n, v1 = i0 + 1 < n;
+    double th0[D], th1[D];
+#pragma unroll
+    for (int j = 0; j < D; j++) {
+        th0[j] = (v0 && j < d) ? theta[i0 * d + j] : 0.0;
+        th1[j] = (v1 && j < d) ? theta[(i0 + 1) * d + j] : 0.0;
+    }
+    double w0 = v0 ? lw[i0] : 0.0, w1 = v1 ? lw[i0 + 1] : 0.0;
+    double p0 = 0.0, p1 = 0.0, q0 = 0.0, q1 = 0.0;
+    if (COMMIT && lpost) { p0 = v0 ? lpost[i0] : 0.0; p1 = v1 ? lpost[i0 + 1] : 0.0; }
+    if (COMMIT && llik) { q0 = v0 ? llik[i0] : 0.0; q1 = v1 ? llik[i0 + 1] : 0.0; }
+    for (int64_t k0 = 0; k0 < K; k0 += kRowsPerTile) {
+        const int rows = (int)((K - k0) < kRowsPerTile ? (K - k0) : kRowsPerTile);
+        __syncthreads();
+        for (int e = threadIdx.x; e < rows * D; e += kSampBlock) {
+            const int r = e / D, j = e - r * D;
+            s_x[e] = (j < d) ? data[(r0 + k0 + r) * d + j] : 0.0;
+        }
+        __syncthreads();
+        for (int r = 0; r < rows; r++) {
+            const double *x = s_x + r * D;
+            double a0 = 0.0, a1 = 0.0;
+#pragma unroll
+            for (int j = 0; j < D; j += 2) {
+                const double2 xx = *reinterpret_cast<const double2 *>(x + j);
+                a0 = fma(th0[j], xx.x, a0); a1 = fma(th1[j], xx.x, a1);
+                a0 = fma(th0[j + 1], xx.y, a0); a1 = fma(th1[j + 1], xx.y, a1);
+            }
+            const double g0 = neg_softplus_neg(a0), g1 = neg_softplus_neg(a1);
+            w0 += g0; w1 += g1;
+            if (w0 != w0) w0 = -CUDART_INF;
+            if (w1 != w1) w1 = -CUDART_INF;
+            if (COMMIT) {
+                p0 += g0; p1 += g1;
+                q0 += g0; q1 += g1;
+            } else {
+                double *row = scratch + (k0 + r) * n;
+                if (v0) row[i0] = w0;
+                if (v1) row[i0 + 1] = w1;
+            }
+        }
+    }
+    if (COMMIT) {
+        if (v0) lw[i0] = w0;
+        if (v1) lw[i0 + 1] = w1;
+        if (lpost && v0) lpost[i0] = p0;
+        if (lpost && v1) lpost[i0 + 1] = p1;
+        if (llik && v0) llik[i0] = q0;
+        if (llik && v1) llik[i0 + 1] = q1;
+    }
+}
+
+}  // namespace smcb
+
+template <int D>
+static int launch_logpyt(smcb_ctx *c, const double *theta, int64_t n, int d, const double *data, int64_t r0,
+                         int64_t K, int commit, double *lw, double *lpost, double *llik, double *scratch) {
+    const int64_t pairs = (n + 1) / 2;
+    const int grid = (int)((pairs + kSampBlock - 1) / kSampBlock);
+    if (commit)
+        LAUNCHK(c, (k_logistic_logpyt<D, true>), grid, kSampBlock, 0, theta, n, d, data, r0, K, lw, lpost, llik,
+                scratch);
+    else
+        LAUNCHK(c, (k_logistic_logpyt<D, false>), grid, kSampBlock, 0, theta, n, d, data, r0, K, lw, lpost, llik,
+                scratch);
+    return SMCB_OK;
+}
+
+// IBIS.logG (smc_samplers.py:773-776) for the logistic-regression model over the rows [r0, r0 + K) of data
+// (n_data, d): commit != 0 adds them to lw / lpost / llik in place, row by row; commit == 0 writes the cumulative
+// log-weights of every row into scratch (K, n) and leaves lw, lpost and llik alone.
+extern "C" int smcb_logistic_logpyt(smcb_ctx *c, const double *theta, int64_t n, int d, const double *data,
+                                    int64_t n_data, int64_t r0, int64_t K, int commit, double *lw, double *lpost,
+                                    double *llik, double *scratch) {
+    SMCB_REQUIRE(c && theta && data && lw && (commit || scratch), "smcb_logistic_logpyt: NULL argument");
+    SMCB_REQUIRE(n >= 1 && d >= 1 && d <= 32, "smcb_logistic_logpyt: need n >= 1 and 1 <= d <= 32");
+    SMCB_REQUIRE(K >= 1 && r0 >= 0 && r0 + K <= n_data, "smcb_logistic_logpyt: rows [%lld, %lld) outside the %lld data rows",
+                 (long long)r0, (long long)(r0 + K), (long long)n_data);
+#define LP(DD) return launch_logpyt<DD>(c, theta, n, d, data, r0, K, commit, lw, lpost, llik, scratch)
+    if (d <= 4) LP(4);
+    if (d <= 8) LP(8);
+    if (d <= 12) LP(12);
+    if (d <= 16) LP(16);
+    if (d <= 20) LP(20);
+    if (d <= 24) LP(24);
+    LP(32);
+#undef LP
+}

@@ -239,10 +239,12 @@ class Beta(ProbDist):
 
 
 class StructDist(ProbDist):
-    """Independent laws of named scalar parameters -- particles/distributions.py:1149-1214.  ``rvs(size)`` returns a
+    """Independent laws of named parameters -- particles/distributions.py:1149-1214.  ``rvs(size)`` returns a
     NumPy structured array (fields in sorted order for a dict, as in the reference), ``logpdf(theta)`` the host
-    array of the summed log-densities.  The component laws may be this package's (device draws, copied to the host)
-    or any object with the same two methods; a callable law (``Cond``) receives the structured array."""
+    array of the summed log-densities.  A law with ``dim > 1`` (``MvNormal``) gets a vector field
+    ``(name, float, (dim,))``; every other law a scalar field.  The component laws may be this package's (device
+    draws, copied to the host) or any object with the same two methods; a callable law (``Cond``) receives the
+    structured array."""
 
     def __init__(self, laws):
         from collections import OrderedDict
@@ -252,7 +254,8 @@ class StructDist(ProbDist):
             self.laws = OrderedDict([(k, laws[k]) for k in sorted(laws)])
         else:
             raise TypeError("recdist class requires a dict or an ordered dict to be instantiated")
-        self.dtype = [(k, float) for k in self.laws]
+        self.dtype = [(k, float) if getattr(law, "dim", 1) == 1 else (k, float, (law.dim,))
+                      for k, law in self.laws.items()]
 
     def logpdf(self, theta):
         lp = 0.0
@@ -265,7 +268,7 @@ class StructDist(ProbDist):
         out = np.empty(size, dtype=self.dtype)
         for par, law in self.laws.items():
             cond = law(out) if callable(law) else law
-            out[par] = _host(cond.rvs(size=size)).reshape(-1)
+            out[par] = _host(cond.rvs(size=size)).reshape(out[par].shape)
         return out
 
 

@@ -1,4 +1,4 @@
-"""SMC samplers on the device: tempering / adaptive tempering with standard or waste-free MCMC
+"""SMC samplers on the device: tempering / adaptive tempering and IBIS with standard or waste-free MCMC
 moves -- the part of ``particles/smc_samplers.py`` that BASELINE config 5 exercises (file:line
 cited per class).  They are Feynman-Kac models for ``particles_b200.SMC`` (plugin path):
 
@@ -87,11 +87,19 @@ class LogisticRegression:
         _lib.check(ctx.lib.smcb_standard_normal(ctx.handle, ptr(z), size * self.d))
         return (self.prior_scale * z).reshape(size, self.d)     # loc + scale * (z @ I)
 
-    def wf_move(self, x, epn, P, noise=None):
+    def _rows(self, n_rows, epn):
+        """(rows, exponent) of the kernels' call for the posterior given the first ``n_rows`` data rows (None: all of
+        them).  No rows is the prior alone: one row at exponent 0, whose log-likelihood the caller then zeroes."""
+        rows = self.T if n_rows is None else int(n_rows)
+        return (1, 0.0) if rows == 0 else (rows, float(epn))
+
+    def wf_move(self, x, epn, P, noise=None, n_rows=None):
         """Fused waste-free move (smcb_logistic_wf_move): x = the M resampled particles with their
-        lprior / llik / lpost at exponent ``epn`` and ``shared['chol_cov']``; returns P*M particles."""
+        lprior / llik / lpost at exponent ``epn`` and ``shared['chol_cov']``; returns P*M particles.
+        ``n_rows``: target the posterior given the first n_rows data rows only (IBIS)."""
         ctx = context()
         M, d = x.theta.shape
+        rows, epn = self._rows(n_rows, epn)
         out = x.__class__(shared=x.shared.copy(), theta=empty((P * M, d)), lprior=empty(P * M),
                           llik=empty(P * M), lpost=empty(P * M))
         pb = empty((P - 1, M))
@@ -99,19 +107,42 @@ class LogisticRegression:
         if noise is not None:
             z, u = as_device(noise[0]), as_device(noise[1])
         _lib.check(ctx.lib.smcb_logistic_wf_move(
-            ctx.handle, M, d, P, ptr(x.theta), ptr(x.lprior), ptr(x.llik), ptr(x.lpost), ptr(self.data), self.T,
-            self.prior_scale, float(epn), ptr(x.shared["chol_cov"]), ptr(z), ptr(u), ptr(out.theta),
+            ctx.handle, M, d, P, ptr(x.theta), ptr(x.lprior), ptr(x.llik), ptr(x.lpost), ptr(self.data), rows,
+            self.prior_scale, epn, ptr(x.shared["chol_cov"]), ptr(z), ptr(u), ptr(out.theta),
             ptr(out.lprior), ptr(out.llik), ptr(out.lpost), ptr(pb)))
+        if n_rows == 0:
+            out.llik.zero_()
         out.shared["acc_rates"] = x.shared.get("acc_rates", []) + [pb.mean(dim=1)]
         return out
 
-    def target(self, x, epn):
+    def target(self, x, epn, n_rows=None):
+        """lprior / llik / lpost of x at exponent ``epn`` (smcb_logistic_target); ``n_rows``: the posterior given
+        the first n_rows data rows only (IBIS.current_target, n_rows = t + 1)."""
         ctx = context()
         n = x.theta.shape[0]
+        rows, epn = self._rows(n_rows, epn)
         x.lprior, x.llik, x.lpost = empty(n), empty(n), empty(n)
-        _lib.check(ctx.lib.smcb_logistic_target(ctx.handle, ptr(x.theta), n, self.d, ptr(self.data), self.T,
-                                                self.prior_scale, float(epn), ptr(x.lprior), ptr(x.llik),
+        _lib.check(ctx.lib.smcb_logistic_target(ctx.handle, ptr(x.theta), n, self.d, ptr(self.data), rows,
+                                                self.prior_scale, epn, ptr(x.lprior), ptr(x.llik),
                                                 ptr(x.lpost)))
+        if n_rows == 0:
+            x.llik.zero_()
+
+    def logpyt_rows(self, theta, r0, K, lw, lpost=None, llik=None, scratch=None):
+        """IBIS reweighting over the data rows [r0, r0 + K) (smcb_logistic_logpyt), one row at a time in row order:
+        with ``scratch`` (K, n), row k receives lw + the rows r0 .. r0 + k and nothing else is written (scan);
+        without it, lw and -- when given -- lpost and llik are incremented in place (commit)."""
+        ctx = context()
+        n = theta.shape[0]
+        _lib.check(ctx.lib.smcb_logistic_logpyt(ctx.handle, ptr(theta), n, self.d, ptr(self.data), self.T, int(r0),
+                                                int(K), int(scratch is None), ptr(lw), ptr(lpost), ptr(llik),
+                                                ptr(scratch)))
+
+    def logpyt(self, theta, t):
+        """log p(y_t | theta) for the (N, d) CUDA tensor theta (StaticModel.logpyt): a one-row commit into zeros."""
+        lpyt = torch.zeros(theta.shape[0], dtype=torch.float64, device=theta.device)
+        self.logpyt_rows(theta, t, 1, lpyt)
+        return lpyt
 
 
 class ArrayRandomWalk:
@@ -312,6 +343,133 @@ class AdaptiveTempering(Tempering):
     def M(self, t, xp):
         xp.shared["rs_flag"] = True
         return self._M(t, xp, xp.shared["exponents"][-1])
+
+
+# ----------------------------------------------------------------------------------------------------------- IBIS
+def _layout(prior):
+    """[(name, column slice)] of the (N, p) theta tensor, from the fields of the prior's structured dtype."""
+    out, j = [], 0
+    dt = np.dtype(prior.dtype)
+    for name in dt.names:
+        k = int(np.prod(dt[name].shape)) if dt[name].shape else 1
+        out.append((name, slice(j, j + k) if dt[name].shape else j))
+        j += k
+    return out
+
+
+class StaticModel:
+    """smc_samplers.py:216-301: a static model given by its data and a ``StructDist`` prior; sub-classes define
+    ``logpyt(theta, t)``.  User code runs on CUDA tensors: ``theta`` is a mapping from field name to a column view
+    of the particles' (N, p) tensor (a (N,) column for a scalar field, (N, dim) for a vector field) and NumPy
+    ``data`` is copied to the device once (``self.data``; the host copy is ``self.data_host``)."""
+
+    def __init__(self, data=None, prior=None):
+        self.data_host = data
+        self.data = as_device(np.asarray(data, dtype=np.float64)) if isinstance(data, np.ndarray) else data
+        self.prior = prior
+
+    @property
+    def T(self):
+        return 0 if self.data is None else len(self.data)
+
+    @property
+    def dim(self):
+        return sum(1 if isinstance(c, int) else c.stop - c.start for _, c in _layout(self.prior))
+
+    def fields(self, theta):
+        """{name: column view} of the (N, p) CUDA tensor theta."""
+        return {name: theta[:, c] for name, c in _layout(self.prior)}
+
+    def logpyt(self, theta, t):
+        raise NotImplementedError("StaticModel: logpyt not implemented")
+
+    def loglik(self, theta, t=None):
+        """Sum of logpyt over the rows 0..t in row order (all rows if t is None), NaN mapped to -inf."""
+        if t is None:
+            t = self.T - 1
+        ll = torch.zeros(theta.shape[0], dtype=torch.float64, device=theta.device)
+        f = self.fields(theta)
+        for s in range(t + 1):
+            ll = ll + as_device(self.logpyt(f, s))
+        return torch.nan_to_num(ll, nan=-float("inf"), posinf=float("inf"), neginf=-float("inf"))
+
+    def logprior(self, theta):
+        """The prior's log-density at the rows of the (N, p) tensor theta, as a CUDA tensor."""
+        return as_device(np.asarray(self.prior.logpdf(self.to_struct(theta)), dtype=np.float64))
+
+    def logpost(self, theta, t=None):
+        return self.logprior(theta) + self.loglik(theta, t)
+
+    def to_struct(self, theta):
+        """(N, p) tensor -> NumPy structured array with the prior's fields."""
+        th = theta.detach().cpu().numpy()
+        out = np.empty(th.shape[0], dtype=self.prior.dtype)
+        for name, c in _layout(self.prior):
+            out[name] = th[:, c]
+        return out
+
+    def prior_rvs(self, size):
+        """Prior draws as the (N, p) CUDA tensor of the particles."""
+        th = self.prior.rvs(size=size)
+        cols = [np.asarray(th[name], dtype=np.float64).reshape(size, -1) for name, _ in _layout(self.prior)]
+        return as_device(np.ascontiguousarray(np.concatenate(cols, axis=1)))
+
+
+def _device_likelihood(model):
+    return hasattr(model, "logpyt_rows")
+
+
+class IBIS(FKSMCsampler):
+    """smc_samplers.py:772-794: data tempering -- the target at step t is the posterior given y_0..y_t.
+
+    ``model`` is a ``StaticModel`` with a user ``logpyt`` (evaluated on CUDA tensors, one call per particle set and
+    data row) or a model with a device likelihood (``LogisticRegression``: reweighting, targets and the waste-free
+    move in libsmcb kernels, no per-row Python).  ``X.theta`` is the (N, d) CUDA tensor.  With a device likelihood,
+    ``SMC.run()`` adds the data rows of a stretch of non-resampling steps with one host read (DESIGN.md 5.10).
+    The adaptive stopping rule of ``AdaptiveMCMCSequence`` is not built; nor is d > 20 (the calibration's bound)."""
+
+    def __init__(self, model=None, wastefree=True, len_chain=10, move=None):
+        super().__init__(model=model, wastefree=wastefree, len_chain=len_chain, move=move)
+        if not _device_likelihood(model) and getattr(type(model), "logpyt", None) in (None, StaticModel.logpyt):
+            raise NotImplementedError("IBIS: model %r has neither a device likelihood nor a logpyt method"
+                                      % type(model).__name__)
+        d = model.d if _device_likelihood(model) else model.dim
+        if d > 20:
+            raise NotImplementedError("IBIS: d = %d parameters; the random-walk calibration is built for d <= 20" % d)
+
+    def logG(self, t, xp, x):
+        if _device_likelihood(self.model):        # a one-row commit: lpost and llik in place, lpyt into zeros
+            lpyt = torch.zeros(x.N, dtype=torch.float64, device=x.theta.device)
+            self.model.logpyt_rows(x.theta, t, 1, lpyt, x.lpost, x.llik)
+            return lpyt
+        lpyt = as_device(self.model.logpyt(self.model.fields(x.theta), t))
+        x.lpost = x.lpost + lpyt
+        x.llik = x.llik + lpyt
+        return lpyt
+
+    def current_target(self, t):
+        model = self.model
+        if _device_likelihood(model):
+            def func(x):
+                model.target(x, 1.0, n_rows=t + 1)
+            func.fused_wf = lambda x, P, noise=None: model.wf_move(x, 1.0, P, noise, n_rows=t + 1)
+            return func
+
+        def func(x):
+            x.lprior = model.logprior(x.theta)
+            x.llik = model.loglik(x.theta, t)
+            x.lpost = x.lprior + x.llik
+        return func
+
+    def _M0(self, N):
+        x0 = ThetaParticles(theta=self.model.prior_rvs(N))
+        self.current_target(-1)(x0)
+        return x0
+
+    def M(self, t, xp):
+        if xp.shared["rs_flag"]:
+            return self.move(xp, self.current_target(t - 1))      # the target at time t - 1: given y_0..y_{t-1}
+        return xp
 
 
 # ---------------------------------------------------------------------------------------------------------- SMC^2
