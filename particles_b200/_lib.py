@@ -83,6 +83,7 @@ class VarDesc(C.Structure):
 
 
 BATCH_AUTO, BATCH_RESIDENT, BATCH_STREAMING = 0, 1, 2
+BATCH_TIERS = {"auto": BATCH_AUTO, "resident": BATCH_RESIDENT, "streaming": BATCH_STREAMING}
 
 
 class BatchDesc(C.Structure):

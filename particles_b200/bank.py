@@ -145,7 +145,7 @@ class FilterBank:
         self.N, self.R, self.T = int(N), int(R), int(data_dev.shape[0])
         self.ld = self.N + (self.N & 1)
         self.data, self.n_params, self.essrmin = data_dev, int(n_params), float(essrmin)
-        self.tier = {"auto": _lib.BATCH_AUTO, "resident": _lib.BATCH_RESIDENT, "streaming": _lib.BATCH_STREAMING}[tier]
+        self.tier = _lib.BATCH_TIERS[tier]
         self._tier_name = tier
         dev = data_dev.device
         f64 = dict(dtype=torch.float64, device=dev)

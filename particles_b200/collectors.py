@@ -443,10 +443,16 @@ class Summaries:
                 col.summary.extend(dict(r) for r in rows)
 
     def _extend_defaults(self, ess, loglt, rs):
-        """Bulk fill from the device table (fused ``run()``)."""
+        """Bulk fill of the default collectors, e.g. with ``default_summaries`` of a device table."""
         self.ESSs.extend(ess)
         self.logLts.extend(loglt)
         self.rs_flags.extend(rs)
+
+
+def default_summaries(table):
+    """Rows of a (T, 4) summary table (ESS, logLt, rs_flag, log_mean_w) -> what the default collectors hold for
+    them: the ESSs and logLts as floats, the rs_flags as bools."""
+    return [float(v) for v in table[:, 0]], [float(v) for v in table[:, 1]], [bool(v) for v in table[:, 2]]
 
 
 def _moments_row(r, dim):

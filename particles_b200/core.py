@@ -66,6 +66,12 @@ def _is_apf(fk):
     return fk.isAPF if hasattr(fk, "isAPF") else ("logeta" in dir(fk))
 
 
+def _stops_at_T(fk):
+    """True when ``fk`` keeps ``FeynmanKac.done`` (ours or the reference's): a run stops after T steps whatever its
+    state, so it may enqueue many steps without a host read per step."""
+    return getattr(getattr(type(fk), "done", None), "__qualname__", "") == "FeynmanKac.done"
+
+
 def fusion_schedule(summaries, N, ESSrmin, mode, batches):
     """What each step-kernel launch of a 1-D single-device fused filter did, replayed on the host from its (T, 4)
     summary table: a list with one entry per step t >= 1, "resample", "plain" (streaming step), "fused" (streaming
@@ -201,6 +207,12 @@ class _FusedEngine:
         _lib.check(self.lib.smcb_filter_state(self.handle, out))
         return list(out)
 
+    def weight_stats(self):
+        """(max, log_mean, ESS, sum exp) of the last step's log-weights, over every shard of a sharded filter: the
+        filter state [.., 4: ESS, 5: log_mean, 6: max, 7: sum exp] as a device tensor laid out as ``Weights._stats``."""
+        st = self.state()
+        return torch.tensor([st[6], st[5], st[4], st[7]], dtype=torch.float64, device=self.lw[0].device)
+
     def fusion_stats(self):
         """Counts of the fused pairs of streaming steps (SMCB_FUSE): launches that ran two steps, launches that
         found their step done, and launches whose pre-computed step resampled after all."""
@@ -293,6 +305,64 @@ def _p2p_pool(ctx, world, rank, group):
     return _pools[key]
 
 
+def _aos(x):
+    """(N, d) view of a component-major (d, N) particle buffer; (N,) buffers as they are."""
+    return x if x.ndim == 1 else x.t()
+
+
+class _Results:
+    """The reference's ``rs_flag, logLt, log_mean_w, loglt, X, Xp, A`` of a device-run filter after ``t`` steps, from
+    ``row(s)``, row s of its (T, 4) summary table (ESS, logLt, rs_flag, log_mean_w) on the host; ``gen(s)``, the (N,)
+    or (d, N) particle buffer step s wrote (steps alternate between two buffers); and ``anc()``, the ancestor buffer,
+    which holds the last step's ancestors when that step resampled."""
+
+    def __init__(self, t, N, row, gen, anc):
+        self.t, self.N = t, N
+        self._row, self._gen, self._anc = row, gen, anc
+
+    @property
+    def rs_flag(self):
+        return False if self.t == 0 else bool(self._row(self.t - 1)[2])
+
+    @property
+    def logLt(self):
+        return 0.0 if self.t == 0 else float(self._row(self.t - 1)[1])
+
+    @property
+    def log_mean_w(self):
+        return float(self._row(self.t - 1)[3])
+
+    @property
+    def loglt(self):
+        if self.t == 1 or self.rs_flag:
+            return self.log_mean_w
+        return self.log_mean_w - float(self._row(self.t - 2)[3])
+
+    @property
+    def X(self):
+        return None if self.t == 0 else _aos(self._gen(self.t - 1))
+
+    @property
+    def A(self):
+        if self.t <= 1:
+            return None
+        A = self._anc()
+        return A if self.rs_flag else torch.arange(self.N, device=A.device)      # core.py:335
+
+    @property
+    def Xp(self):
+        if self.t <= 1:
+            return None
+        prev = self._gen(self.t - 2)
+        if not self.rs_flag:
+            return _aos(prev)
+        out = torch.empty_like(prev)
+        ctx = context(prev.device)
+        _lib.check(ctx.lib.smcb_gather(ctx.handle, ptr(prev), self.N, ptr(self._anc()), self.N,
+                                       1 if prev.ndim == 1 else prev.shape[0], ptr(out)))
+        return _aos(out)
+
+
 class SMC:
     """Drop-in for ``particles.SMC`` (particles/core.py:200-409).
 
@@ -351,21 +421,26 @@ class SMC:
         return self._engine is not None
 
     def _row(self, t):
-        """(ESS, logLt, rs_flag, log_mean_w) of step t from the device table."""
+        """(ESS, logLt, rs_flag, log_mean_w) of step t, read from the device table on first use.  The row read before
+        stays cached as well, so that ``loglt`` (rows t - 1 and t) and ``rs_flag`` (row t) do not evict each other."""
         if t not in self._row_cache:
-            self._row_cache = {t: self._engine.summ[t].cpu().numpy()}
+            self._row_cache = dict(list(self._row_cache.items())[-1:])
+            self._row_cache[t] = self._engine.summ[t].cpu().numpy()
         return self._row_cache[t]
+
+    def _results(self):
+        e = self._engine
+        return _Results(self._done, self.N, self._row, lambda s: e.X[s & 1], lambda: e.A)
 
     def _engine_gen(self, t):
         """Generation t of the fused filter as the on-line smoothers read it, after step t and before step t + 2
         (step s writes buffers [s & 1]): views of the device buffers, and the ancestors chosen on the device from
         the step's resampling flag -- no host sync."""
         e = self._engine
-        x = e.X[t & 1]
         A = None
         if t > 0:
             A = torch.where(e.summ[t, 2] != 0, e.A, torch.arange(self.N, device=e.A.device))
-        return collectors._Gen(t, x if x.ndim == 1 else x.t(), e.lw[t & 1], A)
+        return collectors._Gen(t, _aos(e.X[t & 1]), e.lw[t & 1], A)
 
     def _cur(self):
         return (self._done - 1) & 1      # step s writes buffers [s & 1]
@@ -373,12 +448,7 @@ class SMC:
     # ------------------------------------------------------------- attributes
     @property
     def X(self):
-        if not self.fused:
-            return self._p["X"]
-        if self._done == 0:
-            return None
-        x = self._engine.X[self._cur()]
-        return x if x.ndim == 1 else x.t()          # (N, d) view of the SoA buffer
+        return self._results().X if self.fused else self._p["X"]
 
     @X.setter
     def X(self, v):
@@ -386,55 +456,27 @@ class SMC:
 
     @property
     def rs_flag(self):
-        if not self.fused:
-            return self._p["rs_flag"]
-        return False if self._done == 0 else bool(self._row(self._done - 1)[2])
+        return self._results().rs_flag if self.fused else self._p["rs_flag"]
 
     @property
     def logLt(self):
-        if not self.fused:
-            return self._p["logLt"]
-        return 0.0 if self._done == 0 else float(self._row(self._done - 1)[1])
+        return self._results().logLt if self.fused else self._p["logLt"]
 
     @property
     def log_mean_w(self):
-        if not self.fused:
-            return self._p["log_mean_w"]
-        return float(self._row(self._done - 1)[3])
+        return self._results().log_mean_w if self.fused else self._p["log_mean_w"]
 
     @property
     def loglt(self):
-        if not self.fused:
-            return self._p["loglt"]
-        t = self._done - 1
-        if t == 0 or self.rs_flag:
-            return self.log_mean_w
-        return self.log_mean_w - float(self._engine.summ[t - 1, 3].item())
+        return self._results().loglt if self.fused else self._p["loglt"]
 
     @property
     def A(self):
-        if not self.fused:
-            return self._p["A"]
-        if self._done <= 1:
-            return None
-        if self.rs_flag:
-            return self._engine.A
-        return torch.arange(self.N, device=self._engine.A.device)      # core.py:335
+        return self._results().A if self.fused else self._p["A"]
 
     @property
     def Xp(self):
-        if not self.fused:
-            return self._p["Xp"]
-        if self._done <= 1:
-            return None
-        prev = self._engine.X[self._cur() ^ 1]
-        if not self.rs_flag:
-            return prev if prev.ndim == 1 else prev.t()
-        out = torch.empty_like(prev)
-        ctx = self._engine.ctx
-        _lib.check(ctx.lib.smcb_gather(ctx.handle, ptr(prev), self.N, ptr(self._engine.A), self.N,
-                                       self._engine.dim, ptr(out)))
-        return out if out.ndim == 1 else out.t()
+        return self._results().Xp if self.fused else self._p["Xp"]
 
     @property
     def wgts(self):
@@ -442,10 +484,7 @@ class SMC:
             return self._p["wgts"]
         if self._done == 0:
             return rs.Weights()
-        st = self._engine.state()
-        stats = torch.tensor([st[6], st[5], st[4], st[7]], dtype=torch.float64,
-                             device=self._engine.lw[0].device)
-        return rs.Weights._from_device_stats(self._engine.lw[self._cur()], stats)
+        return rs.Weights._from_device_stats(self._engine.lw[self._cur()], self._engine.weight_stats())
 
     @property
     def aux(self):
@@ -564,7 +603,7 @@ class SMC:
         if self.fused and not self.verbose and not self.hist \
                 and (self.summaries is None or self.summaries.only_defaults or self._dev_moments
                      or len(online) == len(self.summaries._collectors) - self.summaries._n_default) \
-                and getattr(getattr(type(self.fk), "done", None), "__qualname__", "") == "FeynmanKac.done":
+                and _stops_at_T(self.fk):
             T = self._engine.T
             first = self.t
             if online:
@@ -582,9 +621,7 @@ class SMC:
             table = self._engine.summ.cpu().numpy()       # the one device->host read of the run
             self._row_cache = {T - 1: table[T - 1]}
             if self.summaries is not None:
-                self.summaries._extend_defaults([float(v) for v in table[first:T, 0]],
-                                                [float(v) for v in table[first:T, 1]],
-                                                [bool(v) for v in table[first:T, 2]])
+                self.summaries._extend_defaults(*collectors.default_summaries(table[first:T]))
                 if self._dev_moments:
                     self.summaries._extend_moments(self._engine.mom.cpu().numpy()[first:T], self._engine.dim)
                 for col in online:
@@ -608,7 +645,7 @@ class SMC:
         return (isinstance(fk, IBIS) and hasattr(fk.model, "logpyt_rows") and not self.verbose and not self.hist
                 and (self.summaries is None or self.summaries.only_defaults)
                 and type(fk).time_to_resample is FKSMCsampler.time_to_resample
-                and type(fk).done is FeynmanKac.done and not _is_apf(fk))
+                and _stops_at_T(fk) and not _is_apf(fk))
 
     def _run_ibis(self):
         """The per-step loop, with every run of non-resampling steps done as stretches (DESIGN.md section 5.10).
@@ -715,7 +752,7 @@ def batch_key(kw, _specs=None):
     scheme = kw.get("resampling", "systematic")
     if fk is None or scheme not in _lib.FUSED_SCHEMES or N < 1:
         return None, None
-    if getattr(getattr(type(fk), "done", None), "__qualname__", "") != "FeynmanKac.done":
+    if not _stops_at_T(fk):
         return None, None
     from .state_space_models import fused_spec
     if _specs is None:
@@ -738,7 +775,7 @@ def batch_key(kw, _specs=None):
     return key, spec
 
 
-class BatchRun:
+class BatchRun(_Results):
     """One filter of a batched ``multiSMC`` group, after its run: the attributes of ``SMC`` after ``run()``
     (``t, N, fk, logLt, rs_flag, log_mean_w, loglt, X, Xp, A, wgts, W, summaries, cpu_time``) as views of the group's
     device buffers of its chunk.  ``cpu_time`` is the wall time of the chunk (upload, launch, device work and the one
@@ -746,10 +783,12 @@ class BatchRun:
     is built from the chunk's table on first access."""
 
     def __init__(self, buf, i, fk, N, resampling, ESSrmin, seed, table, mom, collect, cpu_time):
+        super().__init__(table.shape[0], N, table.__getitem__, lambda s: buf["X"][i, s & 1, :N],
+                         lambda: buf["A"][i, :N])
         self._buf, self._i = buf, i
-        self.fk, self.N, self.resampling, self.ESSrmin = fk, N, resampling, ESSrmin
+        self.fk, self.resampling, self.ESSrmin = fk, resampling, ESSrmin
         self.qmc, self.verbose, self.hist, self.seed = False, False, None, seed
-        self.T = self.t = table.shape[0]
+        self.T = self.t
         self._table, self._mom, self._collect = table, mom, collect
         self._summaries = None
         self.cpu_time = cpu_time
@@ -758,57 +797,11 @@ class BatchRun:
     def summaries(self):
         if self._summaries is None and self._collect != "off":
             sm = collectors.Summaries(self._collect)
-            t = self._table
-            sm._extend_defaults([float(v) for v in t[:, 0]], [float(v) for v in t[:, 1]], [bool(v) for v in t[:, 2]])
+            sm._extend_defaults(*collectors.default_summaries(self._table))
             if self._mom is not None:
                 sm._extend_moments(self._mom, 1)
             self._summaries = sm
         return self._summaries
-
-    @property
-    def logLt(self):
-        return float(self._table[-1, 1])
-
-    @property
-    def rs_flag(self):
-        return bool(self._table[-1, 2])
-
-    @property
-    def log_mean_w(self):
-        return float(self._table[-1, 3])
-
-    @property
-    def loglt(self):
-        if self.T == 1 or self.rs_flag:
-            return self.log_mean_w
-        return self.log_mean_w - float(self._table[-2, 3])
-
-    def _gen(self, s):
-        return self._buf["X"][self._i, s & 1, :self.N]
-
-    @property
-    def X(self):
-        return self._gen(self.T - 1)
-
-    @property
-    def A(self):
-        if self.T <= 1:
-            return None
-        if self.rs_flag:
-            return self._buf["A"][self._i, :self.N]
-        return torch.arange(self.N, device=self._buf["A"].device)
-
-    @property
-    def Xp(self):
-        if self.T <= 1:
-            return None
-        prev = self._gen(self.T - 2)
-        if not self.rs_flag:
-            return prev
-        ctx = context()
-        out = torch.empty_like(prev)
-        _lib.check(ctx.lib.smcb_gather(ctx.handle, ptr(prev), self.N, ptr(self.A), self.N, 1, ptr(out)))
-        return out
 
     @property
     def wgts(self):
@@ -826,16 +819,21 @@ class BatchRun:
         return self.fk.summary_format(self)
 
 
-def plan_group(key, R, tier="auto"):
-    """(tier, grid) that ``smcb_batch_plan`` chooses for R runs of the group ``key``."""
+def _batch_desc(key, R, tier):
+    """The header of the ``BatchDesc`` of R runs of the group ``key``: kernel selection, tier and shapes."""
     model, fkind, scheme, N, T = key[:5]
     d = _lib.BatchDesc()
     d.model, d.fk, d.scheme, d.dim, d.dy = model, fkind, _lib.RS_CODES[scheme], 1, 1
-    d.tier = {"auto": _lib.BATCH_AUTO, "resident": _lib.BATCH_RESIDENT, "streaming": _lib.BATCH_STREAMING}[tier]
+    d.tier = _lib.BATCH_TIERS[tier]
     d.N, d.T, d.R = N, T, R
+    return d
+
+
+def plan_group(key, R, tier="auto"):
+    """(tier, grid) that ``smcb_batch_plan`` chooses for R runs of the group ``key``."""
     plan = (C.c_int64 * 2)()
     ctx = context()
-    _lib.check(ctx.lib.smcb_batch_plan(ctx.handle, C.byref(d), plan))
+    _lib.check(ctx.lib.smcb_batch_plan(ctx.handle, C.byref(_batch_desc(key, R, tier)), plan))
     return int(plan[0]), int(plan[1])
 
 
@@ -857,20 +855,16 @@ def run_batch(kws, seeds, noise=None, tier="auto", timer=None, out_func=None, _p
         if len(keys) != 1 or None in keys:
             raise ValueError("run_batch: the runs do not form one batchable group")
         key, specs = keys.pop(), [s for _, s in keyed]
-    model, fkind, scheme, N, T, moments, off = key
+    scheme, N, T, moments = key[2:6]
     R, ld = len(kws), N + (N & 1)
     ctx = context()
     ctx.bind_stream()
     dev = ctx.device
     f64 = dict(dtype=torch.float64, device=dev)
     n_params = len(specs[0]["params"])
-    d = _lib.BatchDesc()
-    d.model, d.fk, d.scheme, d.dim, d.dy, d.n_params = model, fkind, _lib.RS_CODES[scheme], 1, 1, n_params
-    d.tier = {"auto": _lib.BATCH_AUTO, "resident": _lib.BATCH_RESIDENT, "streaming": _lib.BATCH_STREAMING}[tier]
-    d.N, d.T, d.R = N, T, R
-    plan = (C.c_int64 * 2)()
-    _lib.check(ctx.lib.smcb_batch_plan(ctx.handle, C.byref(d), plan))
-    streaming = plan[0] == _lib.BATCH_STREAMING
+    streaming = plan_group(key, R, tier)[0] == _lib.BATCH_STREAMING
+    d = _batch_desc(key, R, tier)
+    d.n_params = n_params
     multi = scheme == "multinomial"
     # bytes per run: outputs (X ping-pong, lw, A, summary and moment rows) and inputs (data, step constants, params,
     # seed, ESSrmin, injected noise); the streaming tier's scratch (CDF, spacings) separately

@@ -28,6 +28,7 @@ tests use them to check the scheme itself on CPU with world_size 2.
 import numpy as np
 
 from . import _lib
+from .collectors import default_summaries
 from .core import _FusedEngine
 
 
@@ -79,9 +80,7 @@ class ShardedSMC:
         T = self._engine.T
         self._engine.step(T - self.t)
         table = self._engine.summ.cpu().numpy()      # the one device->host read of the run
-        self.ESSs = [float(v) for v in table[:, 0]]
-        self.logLts = [float(v) for v in table[:, 1]]
-        self.rs_flags = [bool(v) for v in table[:, 2]]
+        self.ESSs, self.logLts, self.rs_flags = default_summaries(table)
         self.t, self.logLt = T, self.logLts[-1]
         self.cpu_time = self._time.perf_counter() - t0
 
@@ -93,11 +92,9 @@ class ShardedSMC:
     def W(self):
         """This rank's slice of the GLOBALLY normalised weights (they sum to one over all ranks): exp(lw - m) / s with
         the (max, sum exp) of all N_global particles that every rank holds after the last step."""
-        import torch
         from .device import context, empty, ptr
-        st = self._engine.state()                     # [.., 4: ESS, 5: log_mean, 6: max, 7: sum exp] of ALL particles
+        stats = self._engine.weight_stats()           # of ALL particles
         lw = self._engine.lw[(self.t - 1) & 1]
-        stats = torch.tensor([st[6], st[5], st[4], st[7]], dtype=torch.float64, device=lw.device)
         W = empty(lw.shape[0], like=lw)
         ctx = context(lw.device)
         _lib.check(ctx.lib.smcb_weights_from_stats(ctx.handle, ptr(lw), lw.shape[0], ptr(stats), ptr(W)))
