@@ -26,11 +26,14 @@ namespace smcb {
 constexpr int kSampBlock = 128;
 constexpr int kRowsPerTile = 32;       // data rows staged in shared memory per pass
 
-// -log(1 + exp(-lin)) = -(max(v, 0) + log1p(exp(-|v|))), v = -lin   (np.logaddexp(0, v))
+// -log(1 + exp(-lin)) = -(max(v, 0) + log1p(exp(-|v|))), v = -lin   (np.logaddexp(0, v)).  A NaN lin (a NaN
+// parameter, or infinite ones whose products cancel) must give NaN, which the row sum turns into -inf as the
+// reference does: fmax drops a NaN and flog_pos reads one as a finite number, so it is passed through explicitly.
 __device__ __forceinline__ double neg_softplus_neg(double lin) {
     const double v = -lin;
     const double e = fexp_neg(-fabs(v));
-    return -(fmax(v, 0.0) + flog_pos(1.0 + e));
+    const double g = -(fmax(v, 0.0) + flog_pos(1.0 + e));
+    return (lin != lin) ? lin : g;
 }
 
 // theta: (n, d) row-major.  D = d rounded up to a supported size (extra coordinates are zero).
