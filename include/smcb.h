@@ -176,6 +176,31 @@ int smcb_logistic_wf_move(smcb_ctx *ctx, int64_t M, int d, int P, const double *
 int smcb_logistic_logpyt(smcb_ctx *ctx, const double *theta, int64_t n, int d, const double *data, int64_t n_data,
                          int64_t r0, int64_t K, int commit, double *lw, double *lpost, double *llik, double *scratch);
 
+/* Nested sampling SMC (NestedSamplingSMC, particles/nested.py:281-373, Salomone et al. 2018) for the same model.
+ * The target is the prior truncated to llik >= lmin (current_target, 353-363): lpost = lprior where llik >= lmin,
+ * -inf elsewhere; lmin = -inf gives the bits of the untempered target (epn = 0).  lmin must not be NaN.
+ * smcb_logistic_ns_target: the arguments of smcb_logistic_target with lmin in place of epn.
+ * smcb_logistic_ns_move: those of smcb_logistic_wf_move with lmin in place of epn; a proposal below the floor has
+ * pb = 0 and is rejected whatever u is.  Same proposals, Philox counters, output order and pb table. */
+int smcb_logistic_ns_target(smcb_ctx *ctx, const double *theta, int64_t n, int d, const double *data,
+                            int64_t n_data, double prior_scale, double lmin, double *lprior, double *llik,
+                            double *lpost);
+int smcb_logistic_ns_move(smcb_ctx *ctx, int64_t M, int d, int P, const double *theta0, const double *lprior0,
+                          const double *llik0, const double *lpost0, const double *data, int64_t n_data,
+                          double prior_scale, double lmin, const double *L_dev, const double *z_in,
+                          const double *u_in, double *theta_out, double *lprior_out, double *llik_out,
+                          double *lpost_out, double *pb_out);
+/* NestedSamplingSMC.logG (nested.py:330-351) in one call, nothing read back inside it.  llik (n): NaN-free.
+ * lt = numpy's _lerp of the order statistics k0 and k1 (k1 = k0 or k0 + 1) of llik with weight gamma: the caller gives
+ * NumPy's "linear" rule, so lt has the bits of np.percentile(llik, 100 (1 - ESSrmin)) (when llik holds both -0.0
+ * and +0.0, a zero lt may carry either sign, as NumPy's partition may).  Then
+ * lZt = t log_alpha - log(n) + logsumexp(llik[llik <= lt]), new_evid = log_sum_exp_ab(log_evid, lZt), the same with
+ * all of llik (new_evid_final, one reduction tree for both), and stop = |new_evid - new_evid_final| < eps.
+ * lw (n): 0 where llik > lt, -inf elsewhere, or all 0 on a stop.  out_dev (3) = (lt, new_evid, stop): (inf,
+ * new_evid_final, 1) on a stop.  10 launches; uses the context's workspace. */
+int smcb_ns_threshold(smcb_ctx *ctx, const double *llik, int64_t n, int64_t k0, int64_t k1, double gamma, int t,
+                      double log_alpha, double log_evid, double eps, double *lw, double *out_dev);
+
 /* AdaptiveTempering's control plane on the device (no host round trip inside a tempering step):
  * next_annealing_epn, smc_samplers.py:876-895: the exponent at which ESS(delta * llik) = alpha * n, by an 11-pass
  * 16-way bracketing search whose state stays in device memory; out_dev[0] = new exponent (1.0 if the whole step fits) */

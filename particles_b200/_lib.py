@@ -164,6 +164,13 @@ PROTOTYPES = {
                                         c_dp, c_dp]),
     "smcb_logistic_logpyt": (C.c_int, [C.c_void_p, c_dp, C.c_int64, C.c_int, c_dp, C.c_int64, C.c_int64, C.c_int64,
                                        C.c_int, c_dp, c_dp, c_dp, c_dp]),
+    "smcb_logistic_ns_target": (C.c_int, [C.c_void_p, c_dp, C.c_int64, C.c_int, c_dp, C.c_int64, C.c_double,
+                                          C.c_double, c_dp, c_dp, c_dp]),
+    "smcb_logistic_ns_move": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp,
+                                        C.c_int64, C.c_double, C.c_double, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
+                                        c_dp, c_dp]),
+    "smcb_ns_threshold": (C.c_int, [C.c_void_p, c_dp, C.c_int64, C.c_int64, C.c_int64, C.c_double, C.c_int,
+                                    C.c_double, C.c_double, C.c_double, c_dp, c_dp]),
     "smcb_rw_propose": (C.c_int, [C.c_void_p, c_dp, C.c_int64, C.c_int, c_dp, c_dp, c_dp]),
     "smcb_mh_accept": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                  c_dp, c_dp]),

@@ -39,7 +39,10 @@ __device__ __forceinline__ double neg_softplus_neg(double lin) {
 // theta: (n, d) row-major.  D = d rounded up to a supported size (extra coordinates are zero).
 // Each thread owns TWO parameter vectors, so every data value read from shared memory feeds two
 // FMAs.  The sum over data rows runs in row order, as the reference's Python loop does.
-template <int D>
+// FLOOR (NestedSamplingSMC.current_target, nested.py:353-363): the argument epn is the likelihood floor lmin
+// and lpost = lprior where llik >= lmin, -inf elsewhere.  Reusing the argument keeps the tempered
+// instantiations' parameter layout, so they compile to the same code as before.
+template <int D, bool FLOOR = false>
 __global__ void __launch_bounds__(kSampBlock) k_logistic_target(
     const double *__restrict__ theta, int64_t n, int d, const double *__restrict__ data, int64_t n_data,
     double prior_scale, double prior_lognorm, double epn, double *__restrict__ lprior,
@@ -87,12 +90,14 @@ __global__ void __launch_bounds__(kSampBlock) k_logistic_target(
     if (v0) {
         const double lp = -0.5 * q0 - prior_lognorm;
         lprior[i0] = lp; llik[i0] = l0;
-        lpost[i0] = (epn > 0.0) ? lp + epn * l0 : lp;        // smc_samplers.py:840-843
+        if (FLOOR) lpost[i0] = (l0 >= epn) ? lp : -CUDART_INF;
+        else lpost[i0] = (epn > 0.0) ? lp + epn * l0 : lp;   // smc_samplers.py:840-843
     }
     if (v1) {
         const double lp = -0.5 * q1 - prior_lognorm;
         lprior[i0 + 1] = lp; llik[i0 + 1] = l1;
-        lpost[i0 + 1] = (epn > 0.0) ? lp + epn * l1 : lp;
+        if (FLOOR) lpost[i0 + 1] = (l1 >= epn) ? lp : -CUDART_INF;
+        else lpost[i0 + 1] = (epn > 0.0) ? lp + epn * l1 : lp;
     }
 }
 
@@ -193,11 +198,13 @@ __global__ void __launch_bounds__(kSampBlock) k_mh_accept(int64_t n, int d, doub
 // kWfLanes lanes of a warp share a chain: each takes every kWfLanes-th data row, a butterfly
 // reduction gives all of them the same log-likelihood bits, so they take the same decision.
 // The data matrix is staged in shared memory once per CTA when it fits (it is re-used P-1 times).
+// FLOOR: the target of nested sampling SMC, the prior truncated to llik >= lmin, with lmin passed as epn (as in
+// k_logistic_target): a proposal below the floor has lpost = -inf, so pb = 0 and it is rejected whatever u is.
 // ---------------------------------------------------------------------------
 constexpr int kWfBlock = 512;
 constexpr int kWfLanes = 16;
 
-template <int D>
+template <int D, bool FLOOR = false>
 __global__ void __launch_bounds__(kWfBlock) k_logistic_wf_move(
     int64_t M, int d, int P, const double *__restrict__ theta0, const double *__restrict__ lprior0,
     const double *__restrict__ llik0, const double *__restrict__ lpost0, const double *__restrict__ data,
@@ -283,7 +290,7 @@ __global__ void __launch_bounds__(kWfBlock) k_logistic_wf_move(
 #pragma unroll
         for (int j = 0; j < D; j++) { const double zz = pr[j] / prior_scale; q += zz * zz; }
         const double lprp = -0.5 * q - prior_lognorm;
-        const double lpp = (epn > 0.0) ? lprp + epn * llp : lprp;
+        const double lpp = FLOOR ? ((llp >= epn) ? lprp : -CUDART_INF) : (epn > 0.0) ? lprp + epn * llp : lprp;
         const double lp_acc = lpp - lp + 0.0;
         double pb = exp(fmin(lp_acc, 0.0));
         if (lp_acc != lp_acc) pb = CUDART_NAN;
@@ -311,7 +318,7 @@ __global__ void __launch_bounds__(kWfBlock) k_logistic_wf_move(
 
 }  // namespace smcb
 
-template <int D>
+template <int D, bool FLOOR>
 static int launch_wf(smcb_ctx *c, int64_t M, int d, int P, const double *theta0, const double *lprior0,
                      const double *llik0, const double *lpost0, const double *data, int64_t n_data, double s,
                      double lognorm, double epn, const double *L, const double *z_in, const double *u_in,
@@ -321,14 +328,38 @@ static int launch_wf(smcb_ctx *c, int64_t M, int d, int P, const double *theta0,
     int64_t tile_rows = (int64_t)((budget - fixed) / (D * sizeof(double)));
     if (tile_rows > n_data) tile_rows = n_data;
     const size_t smem = fixed + (size_t)tile_rows * D * sizeof(double);
-    SMCB_CUDA(cudaFuncSetAttribute(k_logistic_wf_move<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SMCB_CUDA(cudaFuncSetAttribute(k_logistic_wf_move<D, FLOOR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int chains_per_block = kWfBlock / kWfLanes;
     const int grid = (int)((M + chains_per_block - 1) / chains_per_block);
     const uint64_t call = (z_in && u_in) ? 0 : c->api_counter++;
-    LAUNCHK(c, k_logistic_wf_move<D>, grid, kWfBlock, smem, M, d, P, theta0, lprior0, llik0, lpost0, data, n_data,
+    LAUNCHK(c, (k_logistic_wf_move<D, FLOOR>), grid, kWfBlock, smem, M, d, P, theta0, lprior0, llik0, lpost0, data, n_data,
             (int)tile_rows, s, lognorm, epn, L, key_of(c->seed), call, z_in, u_in, theta_out, lprior_out, llik_out,
             lpost_out, pb_out);
     return SMCB_OK;
+}
+
+template <bool FLOOR>
+static int logistic_wf_move(smcb_ctx *c, int64_t M, int d, int P, const double *theta0, const double *lprior0,
+                            const double *llik0, const double *lpost0, const double *data, int64_t n_data,
+                            double prior_scale, double epn, const double *L_dev, const double *z_in,
+                            const double *u_in, double *theta_out, double *lprior_out, double *llik_out,
+                            double *lpost_out, double *pb_out) {
+    SMCB_REQUIRE(c && theta0 && lprior0 && llik0 && lpost0 && data && L_dev && theta_out && lprior_out &&
+                     llik_out && lpost_out && pb_out, "smcb_logistic_wf_move: NULL argument");
+    SMCB_REQUIRE(M >= 1 && P >= 2 && n_data >= 1 && d >= 1 && d <= 32, "smcb_logistic_wf_move: bad sizes");
+    SMCB_REQUIRE(P < 65536, "smcb_logistic_wf_move: len_chain must be < 65536");
+    const double lognorm = (double)d * log(prior_scale) + 0.0 + (double)d * kHalfLog2Pi;
+#define WF(DD) return launch_wf<DD, FLOOR>(c, M, d, P, theta0, lprior0, llik0, lpost0, data, n_data, prior_scale, \
+                                           lognorm, epn, L_dev, z_in, u_in, theta_out, lprior_out, llik_out, lpost_out, \
+                                           pb_out)
+    if (d <= 4) WF(4);
+    if (d <= 8) WF(8);
+    if (d <= 12) WF(12);
+    if (d <= 16) WF(16);
+    if (d <= 20) WF(20);
+    if (d <= 24) WF(24);
+    WF(32);
+#undef WF
 }
 
 // MCMCSequenceWF.__call__ (smc_samplers.py:672-683) for the logistic model + random-walk Metropolis:
@@ -340,32 +371,49 @@ extern "C" int smcb_logistic_wf_move(smcb_ctx *c, int64_t M, int d, int P, const
                                      const double *L_dev, const double *z_in, const double *u_in,
                                      double *theta_out, double *lprior_out, double *llik_out,
                                      double *lpost_out, double *pb_out) {
-    SMCB_REQUIRE(c && theta0 && lprior0 && llik0 && lpost0 && data && L_dev && theta_out && lprior_out &&
-                     llik_out && lpost_out && pb_out, "smcb_logistic_wf_move: NULL argument");
-    SMCB_REQUIRE(M >= 1 && P >= 2 && n_data >= 1 && d >= 1 && d <= 32, "smcb_logistic_wf_move: bad sizes");
-    SMCB_REQUIRE(P < 65536, "smcb_logistic_wf_move: len_chain must be < 65536");
-    const double lognorm = (double)d * log(prior_scale) + 0.0 + (double)d * kHalfLog2Pi;
-#define WF(DD) return launch_wf<DD>(c, M, d, P, theta0, lprior0, llik0, lpost0, data, n_data, prior_scale, lognorm, \
-                                    epn, L_dev, z_in, u_in, theta_out, lprior_out, llik_out, lpost_out, pb_out)
-    if (d <= 4) WF(4);
-    if (d <= 8) WF(8);
-    if (d <= 12) WF(12);
-    if (d <= 16) WF(16);
-    if (d <= 20) WF(20);
-    if (d <= 24) WF(24);
-    WF(32);
-#undef WF
+    return logistic_wf_move<false>(c, M, d, P, theta0, lprior0, llik0, lpost0, data, n_data, prior_scale, epn, L_dev,
+                                   z_in, u_in, theta_out, lprior_out, llik_out, lpost_out, pb_out);
 }
 
-template <int D>
+// The same move under the target of NestedSamplingSMC (nested.py:353-373): the prior truncated to llik >= lmin.
+extern "C" int smcb_logistic_ns_move(smcb_ctx *c, int64_t M, int d, int P, const double *theta0,
+                                     const double *lprior0, const double *llik0, const double *lpost0,
+                                     const double *data, int64_t n_data, double prior_scale, double lmin,
+                                     const double *L_dev, const double *z_in, const double *u_in,
+                                     double *theta_out, double *lprior_out, double *llik_out,
+                                     double *lpost_out, double *pb_out) {
+    SMCB_REQUIRE(lmin == lmin, "smcb_logistic_ns_move: lmin is NaN");
+    return logistic_wf_move<true>(c, M, d, P, theta0, lprior0, llik0, lpost0, data, n_data, prior_scale, lmin, L_dev,
+                                  z_in, u_in, theta_out, lprior_out, llik_out, lpost_out, pb_out);
+}
+
+template <int D, bool FLOOR>
 static int launch_target(smcb_ctx *c, const double *theta, int64_t n, int d, const double *data,
                          int64_t n_data, double s, double lognorm, double epn, double *lprior, double *llik,
                          double *lpost) {
     const int64_t pairs = (n + 1) / 2;
     const int grid = (int)((pairs + kSampBlock - 1) / kSampBlock);
-    LAUNCHK(c, k_logistic_target<D>, grid, kSampBlock, 0, theta, n, d, data, n_data, s, lognorm, epn, lprior,
+    LAUNCHK(c, (k_logistic_target<D, FLOOR>), grid, kSampBlock, 0, theta, n, d, data, n_data, s, lognorm, epn, lprior,
             llik, lpost);
     return SMCB_OK;
+}
+
+template <bool FLOOR>
+static int logistic_target(smcb_ctx *c, const double *theta, int64_t n, int d, const double *data, int64_t n_data,
+                           double prior_scale, double epn, double *lprior, double *llik, double *lpost) {
+    SMCB_REQUIRE(c && theta && data && lprior && llik && lpost, "smcb_logistic_target: NULL argument");
+    SMCB_REQUIRE(n >= 1 && n_data >= 1 && d >= 1 && d <= 32, "smcb_logistic_target: need 1 <= d <= 32");
+    SMCB_REQUIRE(prior_scale > 0.0, "smcb_logistic_target: prior scale must be positive");
+    const double lognorm = (double)d * log(prior_scale) + 0.0 + (double)d * kHalfLog2Pi;
+#define TG(DD) return launch_target<DD, FLOOR>(c, theta, n, d, data, n_data, prior_scale, lognorm, epn, lprior, llik, lpost)
+    if (d <= 4) TG(4);
+    if (d <= 8) TG(8);
+    if (d <= 12) TG(12);
+    if (d <= 16) TG(16);
+    if (d <= 20) TG(20);
+    if (d <= 24) TG(24);
+    TG(32);
+#undef TG
 }
 
 // Tempering.current_target (smc_samplers.py:836-845) for the logistic-regression model with an
@@ -373,17 +421,15 @@ static int launch_target(smcb_ctx *c, const double *theta, int64_t n, int d, con
 extern "C" int smcb_logistic_target(smcb_ctx *c, const double *theta, int64_t n, int d, const double *data,
                                     int64_t n_data, double prior_scale, double epn, double *lprior,
                                     double *llik, double *lpost) {
-    SMCB_REQUIRE(c && theta && data && lprior && llik && lpost, "smcb_logistic_target: NULL argument");
-    SMCB_REQUIRE(n >= 1 && n_data >= 1 && d >= 1 && d <= 32, "smcb_logistic_target: need 1 <= d <= 32");
-    SMCB_REQUIRE(prior_scale > 0.0, "smcb_logistic_target: prior scale must be positive");
-    const double lognorm = (double)d * log(prior_scale) + 0.0 + (double)d * kHalfLog2Pi;
-    if (d <= 4) return launch_target<4>(c, theta, n, d, data, n_data, prior_scale, lognorm, epn, lprior, llik, lpost);
-    if (d <= 8) return launch_target<8>(c, theta, n, d, data, n_data, prior_scale, lognorm, epn, lprior, llik, lpost);
-    if (d <= 12) return launch_target<12>(c, theta, n, d, data, n_data, prior_scale, lognorm, epn, lprior, llik, lpost);
-    if (d <= 16) return launch_target<16>(c, theta, n, d, data, n_data, prior_scale, lognorm, epn, lprior, llik, lpost);
-    if (d <= 20) return launch_target<20>(c, theta, n, d, data, n_data, prior_scale, lognorm, epn, lprior, llik, lpost);
-    if (d <= 24) return launch_target<24>(c, theta, n, d, data, n_data, prior_scale, lognorm, epn, lprior, llik, lpost);
-    return launch_target<32>(c, theta, n, d, data, n_data, prior_scale, lognorm, epn, lprior, llik, lpost);
+    return logistic_target<false>(c, theta, n, d, data, n_data, prior_scale, epn, lprior, llik, lpost);
+}
+
+// NestedSamplingSMC.current_target (nested.py:353-363) for the same model: lpost = lprior where llik >= lmin, else -inf.
+extern "C" int smcb_logistic_ns_target(smcb_ctx *c, const double *theta, int64_t n, int d, const double *data,
+                                       int64_t n_data, double prior_scale, double lmin, double *lprior,
+                                       double *llik, double *lpost) {
+    SMCB_REQUIRE(lmin == lmin, "smcb_logistic_ns_target: lmin is NaN");
+    return logistic_target<true>(c, theta, n, d, data, n_data, prior_scale, lmin, lprior, llik, lpost);
 }
 
 // ArrayRandomWalk.proposal (smc_samplers.py:624-629); L: DEVICE (d, d) row-major lower factor

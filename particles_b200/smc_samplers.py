@@ -93,10 +93,11 @@ class LogisticRegression:
         rows = self.T if n_rows is None else int(n_rows)
         return (1, 0.0) if rows == 0 else (rows, float(epn))
 
-    def wf_move(self, x, epn, P, noise=None, n_rows=None):
+    def wf_move(self, x, epn, P, noise=None, n_rows=None, lmin=None):
         """Fused waste-free move (smcb_logistic_wf_move): x = the M resampled particles with their
         lprior / llik / lpost at exponent ``epn`` and ``shared['chol_cov']``; returns P*M particles.
-        ``n_rows``: target the posterior given the first n_rows data rows only (IBIS)."""
+        ``n_rows``: target the posterior given the first n_rows data rows only (IBIS).  ``lmin``: target the prior
+        truncated to llik >= lmin instead (nested sampling SMC, smcb_logistic_ns_move; ``epn`` is then unused)."""
         ctx = context()
         M, d = x.theta.shape
         rows, epn = self._rows(n_rows, epn)
@@ -106,25 +107,27 @@ class LogisticRegression:
         z = u = None
         if noise is not None:
             z, u = as_device(noise[0]), as_device(noise[1])
-        _lib.check(ctx.lib.smcb_logistic_wf_move(
+        move = ctx.lib.smcb_logistic_wf_move if lmin is None else ctx.lib.smcb_logistic_ns_move
+        _lib.check(move(
             ctx.handle, M, d, P, ptr(x.theta), ptr(x.lprior), ptr(x.llik), ptr(x.lpost), ptr(self.data), rows,
-            self.prior_scale, epn, ptr(x.shared["chol_cov"]), ptr(z), ptr(u), ptr(out.theta),
-            ptr(out.lprior), ptr(out.llik), ptr(out.lpost), ptr(pb)))
+            self.prior_scale, epn if lmin is None else float(lmin), ptr(x.shared["chol_cov"]), ptr(z), ptr(u),
+            ptr(out.theta), ptr(out.lprior), ptr(out.llik), ptr(out.lpost), ptr(pb)))
         if n_rows == 0:
             out.llik.zero_()
         out.shared["acc_rates"] = x.shared.get("acc_rates", []) + [pb.mean(dim=1)]
         return out
 
-    def target(self, x, epn, n_rows=None):
+    def target(self, x, epn, n_rows=None, lmin=None):
         """lprior / llik / lpost of x at exponent ``epn`` (smcb_logistic_target); ``n_rows``: the posterior given
-        the first n_rows data rows only (IBIS.current_target, n_rows = t + 1)."""
+        the first n_rows data rows only (IBIS.current_target, n_rows = t + 1); ``lmin``: lpost = lprior where
+        llik >= lmin, -inf elsewhere instead (NestedSamplingSMC.current_target, smcb_logistic_ns_target)."""
         ctx = context()
         n = x.theta.shape[0]
         rows, epn = self._rows(n_rows, epn)
         x.lprior, x.llik, x.lpost = empty(n), empty(n), empty(n)
-        _lib.check(ctx.lib.smcb_logistic_target(ctx.handle, ptr(x.theta), n, self.d, ptr(self.data), rows,
-                                                self.prior_scale, epn, ptr(x.lprior), ptr(x.llik),
-                                                ptr(x.lpost)))
+        target = ctx.lib.smcb_logistic_target if lmin is None else ctx.lib.smcb_logistic_ns_target
+        _lib.check(target(ctx.handle, ptr(x.theta), n, self.d, ptr(self.data), rows, self.prior_scale,
+                          epn if lmin is None else float(lmin), ptr(x.lprior), ptr(x.llik), ptr(x.lpost)))
         if n_rows == 0:
             x.llik.zero_()
 
