@@ -201,6 +201,43 @@ int smcb_logistic_ns_move(smcb_ctx *ctx, int64_t M, int d, int P, const double *
 int smcb_ns_threshold(smcb_ctx *ctx, const double *llik, int64_t n, int64_t k0, int64_t k1, double gamma, int t,
                       double log_alpha, double log_evid, double eps, double *lw, double *out_dev);
 
+/* SMC samplers on {0,1}^p (particles/binary_smc.py): Bayesian variable selection, p <= 128.  Particles are (n, p)
+ * bytes 0 / 1 (torch.bool).  The model: loglik(gamma) = -(coef_len |gamma| + [use_ldet] ldet + coef_log
+ * log(coef_in_log - gw wtw)) (BIC 227-230, BayesianVS 258-265 with use_ldet = 1, BayesianVS_gprior 287-293 with
+ * gw = g / (g + 1)), prior IID(Bernoulli(q), p) with lq = log(clip(q)), l1q = log(clip(1 - q)). */
+typedef struct {
+    int32_t p;                 /* predictors, 1..128                                                     */
+    int32_t use_ldet;          /* 1: the log-determinant enters loglik (BayesianVS)                      */
+    const double *xtx;         /* (p, p) device, X^T X                                                   */
+    const double *xty;         /* (p) device, X^T y                                                      */
+    double vm2;                /* added to the diagonal of X^T X[gamma, gamma] by the move (iv2)         */
+    double coef_len, coef_log, coef_in_log, gw;
+    double lq, l1q;
+} smcb_vs_desc;
+
+/* chol_and_friends (binary_smc.py:165-180) with diagonal shift vm2 for the n rows of gamma: len_gam, ldet =
+ * sum log diag L, wtw = |L^-1 X^T y[gamma]|^2 ((0, 0, 0) for an empty gamma); each output may be NULL.  llik (or
+ * NULL): the model's loglik; lprior and lpost (or NULL; lpost needs both): the prior and lprior + epn llik
+ * (lprior where epn <= 0).  kmax >= every |gamma| (it sizes shared memory).  *err (device int, zeroed by the
+ * caller): bit 0 = a non-positive pivot (that row gets llik = -inf, ldet = wtw = NaN), bit 1 = a row above kmax. */
+int smcb_vs_loglik(smcb_ctx *ctx, const smcb_vs_desc *model, const uint8_t *gamma, int64_t n, int kmax, double vm2,
+                   double epn, double *len_gam, double *ldet, double *wtw, double *lprior, double *llik,
+                   double *lpost, int *err);
+/* NestedLogistic (binary_smc.py:83-118) with device coeffs (p, p) and edgy (p): draw != 0: x (n, p) := rvs, from
+ * u_in (p, n) (the reference's order of draws) or the context's Philox stream; logpdf (or NULL) = its log-density.
+ * draw == 0: logpdf of the given x. */
+int smcb_nested_logistic(smcb_ctx *ctx, int p, const double *coeffs, const uint8_t *edgy, int64_t n, int draw,
+                         uint8_t *x, const double *u_in, double *logpdf);
+/* MCMCSequenceWF.__call__ (smc_samplers.py:672-683) with BinaryMetropolis (binary_smc.py:154-162) under the tempered
+ * target at exponent epn: ONE launch runs the P-1 steps of all M chains.  Inputs: the M resampled particles with
+ * their lprior / llik / lpost; outputs: the P*M particles in concatenate(xs) order and pb_out (P-1, M), the
+ * acceptance probabilities.  u_prop (P-1, p, M) and u_acc (P-1, M): injected uniforms, or both NULL.  *err as for
+ * smcb_vs_loglik (bit 0). */
+int smcb_binary_wf_move(smcb_ctx *ctx, const smcb_vs_desc *model, const double *coeffs, const uint8_t *edgy,
+                        int64_t M, int P, double epn, const uint8_t *x0, const double *lprior0, const double *llik0,
+                        const double *lpost0, const double *u_prop, const double *u_acc, uint8_t *x_out,
+                        double *lprior_out, double *llik_out, double *lpost_out, double *pb_out, int *err);
+
 /* AdaptiveTempering's control plane on the device (no host round trip inside a tempering step):
  * next_annealing_epn, smc_samplers.py:876-895: the exponent at which ESS(delta * llik) = alpha * n, by an 11-pass
  * 16-way bracketing search whose state stays in device memory; out_dev[0] = new exponent (1.0 if the whole step fits) */

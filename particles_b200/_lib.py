@@ -127,6 +127,14 @@ class CsmcDesc(C.Structure):
     ]
 
 
+class VsDesc(C.Structure):
+    _fields_ = [
+        ("p", C.c_int32), ("use_ldet", C.c_int32), ("xtx", c_dp), ("xty", c_dp), ("vm2", C.c_double),
+        ("coef_len", C.c_double), ("coef_log", C.c_double), ("coef_in_log", C.c_double), ("gw", C.c_double),
+        ("lq", C.c_double), ("l1q", C.c_double),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/smcb.h declares
 PROTOTYPES = {
     "smcb_last_error": (C.c_char_p, []),
@@ -171,6 +179,11 @@ PROTOTYPES = {
                                         c_dp, c_dp]),
     "smcb_ns_threshold": (C.c_int, [C.c_void_p, c_dp, C.c_int64, C.c_int64, C.c_int64, C.c_double, C.c_int,
                                     C.c_double, C.c_double, C.c_double, c_dp, c_dp]),
+    "smcb_vs_loglik": (C.c_int, [C.c_void_p, C.POINTER(VsDesc), c_dp, C.c_int64, C.c_int, C.c_double, C.c_double,
+                                 c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp]),
+    "smcb_nested_logistic": (C.c_int, [C.c_void_p, C.c_int, c_dp, c_dp, C.c_int64, C.c_int, c_dp, c_dp, c_dp]),
+    "smcb_binary_wf_move": (C.c_int, [C.c_void_p, C.POINTER(VsDesc), c_dp, c_dp, C.c_int64, C.c_int, C.c_double,
+                                      c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp]),
     "smcb_rw_propose": (C.c_int, [C.c_void_p, c_dp, C.c_int64, C.c_int, c_dp, c_dp, c_dp]),
     "smcb_mh_accept": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
                                  c_dp, c_dp]),

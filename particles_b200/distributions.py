@@ -390,6 +390,28 @@ class IndepProd(ProbDist):
         return torch.stack(cols, dim=1)
 
 
+class IID(IndepProd):
+    """Joint law of k iid copies of ``law`` -- particles/distributions.py:1111-1121 (there IndepProd(*[law] * k));
+    (N, k) inputs / outputs.  A law with a joint device kernel for its iid product (``binary_smc.Bernoulli``) is
+    drawn and evaluated by that kernel, in the reference's order of draws and terms."""
+
+    def __init__(self, law, k):
+        super().__init__(*[law for _ in range(k)])
+        self.law = law
+
+    def rvs(self, size=None, z=None):
+        joint = getattr(self.law, "_iid", None)
+        if joint is not None:
+            return joint(self.dim).rvs(size=1 if size is None else size)
+        return super().rvs(size=size, z=z)
+
+    def logpdf(self, x):
+        joint = getattr(self.law, "_iid", None)
+        if joint is not None:
+            return joint(self.dim).logpdf(x)
+        return super().logpdf(x)
+
+
 class MvNormal(ProbDist):
     """Multivariate Normal -- particles/distributions.py:888-982 (d <= 32 on the device).
     ``loc``: (d,) or (N, d); ``scale``: scalar, (d,) or (N, d); ``cov``: (d, d) host array."""

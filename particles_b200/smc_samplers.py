@@ -20,6 +20,7 @@ from scipy import optimize
 
 from . import _lib
 from . import resampling as rs
+from .binary_smc import BinaryMetropolis
 from .core import FeynmanKac
 from .device import as_device, context, empty, ptr
 
@@ -48,6 +49,9 @@ class ThetaParticles:
         ctx = context(key.device)
         out = {}
         for k, v in self.dict_fields.items():
+            if v.dtype != torch.float64:          # e.g. the (N, p) bool theta of binary_smc: a plain row copy
+                out[k] = v.index_select(0, key)
+                continue
             d = 1 if v.ndim == 1 else v.shape[1]
             o = torch.empty((key.shape[0],) + tuple(v.shape[1:]), dtype=v.dtype, device=v.device)
             _lib.check(ctx.lib.smcb_gather_rows(ctx.handle, ptr(v), v.shape[0], ptr(key), key.shape[0], d,
@@ -194,7 +198,7 @@ class MCMCSequenceWF(MCMCSequence):
 
     def __call__(self, x, target, noise=None):
         fused = getattr(target, "fused_wf", None)
-        if fused is not None and isinstance(self.mcmc, ArrayRandomWalk) and self.nsteps >= 1:
+        if fused is not None and isinstance(self.mcmc, (ArrayRandomWalk, BinaryMetropolis)) and self.nsteps >= 1:
             return fused(x, self.nsteps + 1, noise)     # all chains, all steps: one kernel launch
         xs, ars = [x], []
         for _ in range(self.nsteps):
