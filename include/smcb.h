@@ -443,6 +443,43 @@ typedef struct {
 int smcb_online_smooth(smcb_ctx *ctx, const smcb_online_desc *desc);
 
 /* ---------------------------------------------------------------------------
+ * two-filter smoothing (particles/smoothing.py:487-566) of a forward generation X_t (N particles, log-weights lw)
+ * against an information generation Xinfo (Ninfo particles), one-dimensional states only; the pair density is
+ * logpt(t + 1, X_t[n], Xinfo[m]).  The caller evaluates the user's phi between the launches and combines the rows
+ * (exp_and_normalise of lwinfo + L, dotted with S).
+ * ------------------------------------------------------------------------- */
+#define SMCB_TF_ON2_ROWS 0  /* rows [row0, row0 + rows) of Xinfo, one pass over n, omega never stored:
+                               L[m] = log sum_n exp(v_nm), S[m] = sum_n exp(v_nm - L[m]) psi[m - row0, n],
+                               v_nm = lw[n] + logpt(t + 1, X_t[n], Xinfo[m]); a row with no positive pair weight
+                               gives L = -inf, S = 0.  Partial sums merge in a fixed order (bits = f(inputs)) */
+#define SMCB_TF_ON_LOGW 1   /* one thread per draw j: log_omega[j] = logpt(t + 1, X_t[J[j]], Xinfo[I[j]])
+                               - mf[J[j]] - mi[I[j]] (mf, mi may be NULL); xf[j] = X_t[J[j]], xi[j] = Xinfo[I[j]] */
+
+typedef struct {
+    int32_t method, model, dim, n_params;
+    int64_t t;                 /* forward time; the density is logpt(t + 1, X_t, Xinfo)                  */
+    int64_t N, Ninfo;          /* particles of X_t and of Xinfo                                          */
+    int64_t row0, rows;        /* ON2_ROWS: the block of rows of Xinfo                                   */
+    int64_t M;                 /* ON_LOGW: draws                                                         */
+    double step_const;         /* the model's per-step constant of step t + 1 (Gordon_etal), else 0      */
+    double params[SMCB_MAX_PARAMS];  /* model constants, same layout as smcb_filter_desc.params          */
+    /* particle n at X[n * x_stride], m at Xinfo[m * xi_stride] (element strides)                        */
+    const double *X;
+    const double *Xinfo;
+    int64_t x_stride, xi_stride;
+    const double *lw;          /* ON2_ROWS: (N) forward log-weights at t                                 */
+    const double *psi;         /* ON2_ROWS: (rows, N) phi(X_t[n], Xinfo[row0 + r]) at [r, n]             */
+    double *L, *S;             /* ON2_ROWS: out (Ninfo), rows [row0, row0 + rows) written               */
+    const int64_t *I, *J;      /* ON_LOGW: (M) indices into Xinfo and X_t (in range: not checked)        */
+    const double *mf, *mi;     /* ON_LOGW: NULL or (N) / (Ninfo) log-modifiers                           */
+    double *log_omega;         /* ON_LOGW: out (M)                                                       */
+    double *xf, *xi;           /* ON_LOGW: out (M) the gathered pairs                                    */
+} smcb_twofilter_desc;
+
+/* one kernel launch, no host sync; a model whose state is not one-dimensional -> SMCB_ENOSYS */
+int smcb_two_filter(smcb_ctx *ctx, const smcb_twofilter_desc *desc);
+
+/* ---------------------------------------------------------------------------
  * genealogy-based variance estimators (particles/variance_estimators.py:93-201): the Eve indices of a running filter
  * and the branch sums  sum_b (sum_{m: B_m = b} v_m)^2  over SORTED rows B, so that each branch is a contiguous run.
  * ------------------------------------------------------------------------- */

@@ -68,6 +68,20 @@ class OnlineDesc(C.Structure):
     ]
 
 
+TF_ON2_ROWS, TF_ON_LOGW = 0, 1
+
+
+class TwoFilterDesc(C.Structure):
+    _fields_ = [
+        ("method", C.c_int32), ("model", C.c_int32), ("dim", C.c_int32), ("n_params", C.c_int32),
+        ("t", C.c_int64), ("N", C.c_int64), ("Ninfo", C.c_int64), ("row0", C.c_int64), ("rows", C.c_int64),
+        ("M", C.c_int64), ("step_const", C.c_double), ("params", C.c_double * SMCB_MAX_PARAMS),
+        ("X", c_dp), ("Xinfo", c_dp), ("x_stride", C.c_int64), ("xi_stride", C.c_int64),
+        ("lw", c_dp), ("psi", c_dp), ("L", c_dp), ("S", c_dp), ("I", c_dp), ("J", c_dp), ("mf", c_dp), ("mi", c_dp),
+        ("log_omega", c_dp), ("xf", c_dp), ("xi", c_dp),
+    ]
+
+
 VAR_EVE, VAR_SUMS = 0, 1
 VAR_CENTRED, VAR_WEIGHTS = 0, 1
 
@@ -207,6 +221,7 @@ PROTOTYPES = {
     "smcb_filter_fusion_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "smcb_backward_sample": (C.c_int, [C.c_void_p, C.POINTER(SmoothDesc)]),
     "smcb_online_smooth": (C.c_int, [C.c_void_p, C.POINTER(OnlineDesc)]),
+    "smcb_two_filter": (C.c_int, [C.c_void_p, C.POINTER(TwoFilterDesc)]),
     "smcb_variance": (C.c_int, [C.c_void_p, C.POINTER(VarDesc)]),
     "smcb_variance_scratch_doubles": (C.c_int64, [C.c_int64, C.c_int64, C.c_int64]),
     "smcb_batch_plan": (C.c_int, [C.c_void_p, C.POINTER(BatchDesc), C.POINTER(C.c_int64)]),

@@ -201,11 +201,7 @@ __global__ void __launch_bounds__(kSmBlock) k_on2_weights(M m, smcb_online_desc 
 #pragma unroll
         for (int mask = 16; mask > 0; mask >>= 1) {
             const double mo = __shfl_xor_sync(kFull, mx[r], mask), so = __shfl_xor_sync(kFull, s[r], mask);
-            const double Mx = fmax(mx[r], mo);
-            if (Mx > -CUDART_INF) {
-                s[r] = s[r] * fexp_neg(mx[r] - Mx) + so * fexp_neg(mo - Mx);
-                mx[r] = Mx;
-            }
+            lse_merge(mx[r], s[r], mo, so);
         }
         if (lane == 0) {
             s_part[0][warp][r] = mx[r];

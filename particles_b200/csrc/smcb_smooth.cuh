@@ -58,6 +58,17 @@ __device__ __forceinline__ void lse_add(double &mx, double &s, double v) {
     }
 }
 
+// merge the partial (mo, so) of a disjoint set of values into (mx, s): both rescaled to the larger max, so that s is
+// again sum exp(v - mx); two empty partials (max -inf) stay empty.  A sum of exp(v - mx) * psi kept beside s merges
+// the same way, from a copy of mx taken before.
+__device__ __forceinline__ void lse_merge(double &mx, double &s, double mo, double so) {
+    const double Mx = fmax(mx, mo);
+    if (Mx > -CUDART_INF) {
+        s = s * fexp_neg(mx - Mx) + so * fexp_neg(mo - Mx);
+        mx = Mx;
+    }
+}
+
 template <class M>
 __device__ __forceinline__ void stage_tables(const double *tab, uint64_t *bar, bool needed) {
     if (!needed) return;
@@ -86,11 +97,7 @@ __device__ int64_t warp_exact_draw(const M &m, const TransDensity<M> &td, const 
 #pragma unroll
     for (int mask = 16; mask > 0; mask >>= 1) {
         const double mo = __shfl_xor_sync(kFull, mx, mask), so = __shfl_xor_sync(kFull, s, mask);
-        const double Mx = fmax(mx, mo);
-        if (Mx > -CUDART_INF) {
-            s = s * fexp_neg(mx - Mx) + so * fexp_neg(mo - Mx);
-            mx = Mx;
-        }
+        lse_merge(mx, s, mo, so);
     }
     const double target = u * s;
     double c = 0.0;

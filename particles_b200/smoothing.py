@@ -9,6 +9,10 @@ Backward sampling (``backward_sampling_ON2 / _mcmc / _reject``): when the transi
 ``PX`` (``state_space_models.transition_spec``) the whole backward pass is ONE kernel launch
 (csrc/smcb_smooth.cu); otherwise the same algorithms run with ``fk.logpt`` called on CUDA tensors, with the
 library's sampling, CDF and gather kernels underneath.  There is no CPU path.
+
+Two-filter smoothing (``two_filter_smoothing``, O(N^2) and O(N), one-dimensional states) works the same way:
+csrc/smcb_twofilter.cu on a stock model's transition, ``fk.logpt`` on CUDA tensors otherwise; ``smoothing_worker``
+drives every off-line method as the reference's book scripts do.
 """
 import ctypes as C
 from collections import deque
@@ -19,6 +23,12 @@ import torch
 from . import _lib
 from . import resampling as rs
 from .device import as_device, context, ptr
+
+
+def _flat(x):
+    """A 1-D particle array as the two-filter kernels read it: (N,) fp64 on the device, element stride kept."""
+    x = x if isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float64 else as_device(x)
+    return x.reshape(x.shape[0]) if x.ndim > 1 else x
 
 
 def _own(x):
@@ -152,8 +162,132 @@ class ParticleHistory(RollingParticleHistory):
         raise NotImplementedError("QMC backward sampling needs SQMC (qmc=True), which is outside the "
                                   "accelerated path")
 
-    def two_filter_smoothing(self, *args, **kwargs):
-        raise NotImplementedError("two-filter smoothing is not built in particles_b200")
+    # ------------------------------------------------------------ two-filter
+    def two_filter_smoothing(self, t, info, phi, loggamma, linear_cost=False, return_ess=False,
+                             modif_forward=None, modif_info=None, seed=None, noise=None):
+        """Two-filter estimate of the smoothing expectation of phi(X_t, X_{t+1}), smoothing.py:487-566.
+
+        ``info`` is the information filter: an ``SMC`` run with ``store_history=True`` over the same T (usually the
+        data in reverse), whose generation ti = T-2-t stands for X_{t+1}; ``loggamma`` is the log-density of its
+        'prior' gamma_{t+1}.  One-dimensional states only (d > 1 raises NotImplementedError).
+
+        Calling convention: ``phi(x, xf)`` and ``loggamma(x)`` receive CUDA fp64 tensors -- ``phi`` the two members
+        of each pair as tensors of the same shape -- and return CUDA tensors or arrays of their length; in the O(N^2)
+        method phi must give one value per pair, in the linear one a (K,) or (K, k) array.
+
+        ``linear_cost=False`` (O(N^2)): sum_{n,m} omega_nm phi / sum_{n,m} omega_nm over all pairs, in blocks of at
+        most 2^24 pairs (one kernel launch per block on a stock model's transition, ``fk.logpt`` on the pairs
+        otherwise).  ``linear_cost=True`` (O(N), equal N in both filters): N pairs drawn by multinomial resampling
+        (I from the information weights, then J from the forward ones, each optionally tilted by ``modif_info`` /
+        ``modif_forward``), reweighted by the transition density.  ``return_ess`` also returns 1 / sum Om^2.
+
+        Returns a CUDA fp64 0-d tensor (a (k,) tensor for a vector phi in the linear method); nothing is read back
+        to the host.  ``seed`` re-keys the device generator first; ``noise={"I": ..., "J": ...}`` injects the
+        draws of the linear method (parity tests)."""
+        ti = self.T - 2 - t
+        if t < 0 or t >= self.T - 1:
+            raise ValueError("two-filter smoothing: t must be in range 0,...,T-2")
+        if any(x.ndim > 1 and x.shape[1] != 1 for x in (self.X[t], self.X[t + 1])):
+            raise NotImplementedError("two-filter smoothing is not built for d > 1 (one-dimensional states only)")
+        ih = getattr(info, "hist", None)
+        if not isinstance(ih, ParticleHistory) or ih.T != self.T:
+            raise ValueError("two-filter smoothing: info must be an SMC run with store_history=True over the same "
+                             f"T = {self.T}")
+        x, xi = _flat(self.X[t]), _flat(ih.X[ti])
+        lw = self.wgts[t].lw.contiguous()
+        lwinfo = ih.wgts[ti].lw - as_device(loggamma(xi)).reshape(-1)
+        from .state_space_models import transition_spec
+        spec = transition_spec(self.fk)
+        if linear_cost:
+            return self._two_filter_ON(t, x, xi, lw, lwinfo, phi, spec, return_ess, modif_forward, modif_info,
+                                       seed, noise)
+        return self._two_filter_ON2(t, x, xi, lw, lwinfo, phi, spec)
+
+    def _tf_desc(self, method, spec, t, x_fwd, x_info, **kw):
+        d = _lib.TwoFilterDesc()
+        d.method, d.model, d.dim, d.n_params = method, spec["model"], spec["dim"], len(spec["params"])
+        for i, v in enumerate(spec["params"]):
+            d.params[i] = float(v)
+        sc = spec.get("step_consts")
+        d.step_const = float(sc[t + 1]) if sc is not None else 0.0
+        d.t, d.N, d.Ninfo = t, x_fwd.shape[0], x_info.shape[0]
+        d.X, d.Xinfo = x_fwd.data_ptr(), x_info.data_ptr()
+        d.x_stride, d.xi_stride = x_fwd.stride(0), x_info.stride(0)
+        for k, v in kw.items():
+            setattr(d, k, v.data_ptr() if isinstance(v, torch.Tensor) else v)
+        ctx = context(x_fwd.device)
+        _lib.check(ctx.lib.smcb_two_filter(ctx.handle, C.byref(d)))
+
+    def _two_filter_ON2(self, t, x, xi, lw, lwinfo, phi, spec):
+        """smoothing.py:527-547 by rows m of the information filter: L[m] = log sum_n exp(lw_t[n] + logpt(t+1,
+        X_t[n], Xinfo[m])), S[m] the omega-weighted mean of phi over row m; then exp_and_normalise(lwinfo + L) . S.
+        A row with no positive pair weight contributes exactly 0; no positive weight at all gives NaN (0 / 0)."""
+        from .collectors import _ON2_PAIRS, _repeat_rows, _tile_rows
+        N, Ni = x.shape[0], xi.shape[0]
+        dev = x.device
+        R = max(1, min(Ni, _ON2_PAIRS // N))
+        L = torch.empty(Ni, dtype=torch.float64, device=dev)
+        S = torch.empty(Ni, dtype=torch.float64, device=dev)
+        for r0 in range(0, Ni, R):
+            rows = min(R, Ni - r0)
+            xa, xb = _tile_rows(x, rows), _repeat_rows(xi[r0:r0 + rows], N)      # pair [r, n] = (X_t[n], Xinfo[m])
+            psi = as_device(phi(xa, xb))
+            if psi.numel() != rows * N:
+                raise ValueError("two-filter smoothing (O(N^2)): phi must return one value per pair, got shape "
+                                 f"{tuple(psi.shape)} for {rows * N} pairs")
+            psi = psi.reshape(rows, N).contiguous()
+            if spec is not None:
+                self._tf_desc(_lib.TF_ON2_ROWS, spec, t, x, xi, row0=r0, rows=rows, lw=lw, psi=psi, L=L, S=S)
+            else:                  # fk.logpt on the device tensors of the pairs
+                v = lw[None, :] + as_device(self.fk.logpt(t + 1, xa, xb)).reshape(rows, N)
+                Lb = torch.logsumexp(v, dim=1)
+                L[r0:r0 + rows] = Lb
+                S[r0:r0 + rows] = torch.where(Lb > -np.inf, (torch.softmax(v, dim=1) * psi).sum(1), 0.0)
+        W = rs.exp_and_normalise(lwinfo + L)
+        return (W * S).sum()
+
+    def _two_filter_ON(self, t, x, xi, lw, lwinfo, phi, spec, return_ess, modif_forward, modif_info, seed, noise):
+        """smoothing.py:549-566."""
+        N = x.shape[0]
+        if xi.shape[0] != N:
+            raise ValueError(f"two-filter smoothing (O(N)): the filters must have the same N, got {N} and "
+                             f"{xi.shape[0]}")
+        dev = x.device
+        if seed is not None:
+            context(dev).seed(seed)
+        nz = noise or {}
+        mf = None if modif_forward is None else as_device(modif_forward).reshape(-1).contiguous()
+        mi = None if modif_info is None else as_device(modif_info).reshape(-1).contiguous()
+        if nz.get("I") is not None:
+            I = as_device(nz["I"], dtype=torch.int64, device=dev).reshape(-1)
+        else:
+            I = rs.multinomial(rs.exp_and_normalise(lwinfo if mi is None else lwinfo + mi))
+        if nz.get("J") is not None:
+            J = as_device(nz["J"], dtype=torch.int64, device=dev).reshape(-1)
+        else:
+            J = rs.multinomial(self.wgts[t].W if mf is None else rs.exp_and_normalise(lw + mf))
+        if spec is not None:
+            log_omega, xf, xg = (torch.empty(N, dtype=torch.float64, device=dev) for _ in range(3))
+            self._tf_desc(_lib.TF_ON_LOGW, spec, t, x, xi, M=N, I=I, J=J, mf=0 if mf is None else mf,
+                          mi=0 if mi is None else mi,
+                          log_omega=log_omega, xf=xf, xi=xg)
+        else:
+            xf, xg = x[J], xi[I]
+            log_omega = as_device(self.fk.logpt(t + 1, xf, xg)).reshape(-1)
+            if mf is not None:
+                log_omega = log_omega - mf[J]
+            if mi is not None:
+                log_omega = log_omega - mi[I]
+        Om = rs.exp_and_normalise(log_omega)
+        v = as_device(phi(xf, xg))
+        if v.ndim == 0 or v.shape[0] != N or v.ndim > 2:
+            raise ValueError(f"two-filter smoothing (O(N)): phi must return (N,) or (N, k) with N = {N}, got "
+                             f"{tuple(v.shape)}")
+        w = Om if v.ndim == 1 else Om[:, None]
+        est = (w * v).sum(0) / Om.sum()                      # np.average(phi, axis=0, weights=Om)
+        if return_ess:
+            return est, 1.0 / (Om ** 2).sum()
+        return est
 
     # -------------------------------------------------------------- plumbing
     def _history_desc(self, method, M):
@@ -311,3 +445,78 @@ class ParticleHistory(RollingParticleHistory):
                 self._exact_draw(t, X[t + 1][idx[t + 1, m]], None if u_exact is None else u_exact[t, m], idx[t, m])
             self.acc_rate[t] = (M - nrej) / nprops if nprops else np.nan
         return idx
+
+
+# ---------------------------------------------------------------------------
+# smoothing_worker -- smoothing.py:569-677
+# ---------------------------------------------------------------------------
+_PURE_REJECT_TRIALS = (1 << 24) - 1     # the most proposals per draw the device samplers take (reference: N * 10^9)
+WORKER_METHODS = ("FFBS_purereject", "FFBS_hybrid", "FFBS_MCMC", "FFBS_ON2", "FFBS_QMC",
+                  "two-filter_ON", "two-filter_ON_prop", "two-filter_ON2")
+
+
+def _norm_logpdf(x, loc, scale):
+    """scipy.stats.norm.logpdf(x, loc, scale) on device tensors, in scipy's order of operations."""
+    z = (x - loc) / scale
+    return -z * z / 2.0 - 0.5 * np.log(2.0 * np.pi) - torch.log(scale)
+
+
+def smoothing_worker(method=None, N=100, fk=None, fk_info=None, add_func=None, log_gamma=None):
+    """Generic worker for the off-line smoothing algorithms, smoothing.py:569-677; usable with
+    ``utils.multiplexer``.  Runs the forward filter (and, for the two-filter methods, the information filter
+    ``fk_info``, by default the same model with the data in reverse), then estimates for every t in 0..T-2 the
+    smoothing expectation of ``add_func(t, x, xf)`` (x = X_t, xf = X_{t+1}) with ``method``, one of
+    ``WORKER_METHODS``.  ``add_func`` and ``log_gamma`` receive CUDA fp64 tensors, as ``two_filter_smoothing``'s
+    ``phi`` and ``loggamma`` do.
+
+    Returns {"est": (T-1,) array, "cpu": seconds}: the estimates stay on the device until one read at the end, and
+    ``cpu`` is the wall time of the runs plus the smoothing, ending with that read.  'FFBS_purereject' is the
+    hybrid sampler with 2^24 - 1 proposals per draw before the exact draw (the reference allows N * 10^9);
+    'FFBS_QMC' raises NotImplementedError (SQMC is not built); an unknown method raises ValueError."""
+    import time
+
+    from .core import SMC
+    if method not in WORKER_METHODS:
+        raise ValueError(f"smoothing_worker: no such method {method!r}; one of {WORKER_METHODS}")
+    if method == "FFBS_QMC":
+        raise NotImplementedError("smoothing_worker: FFBS_QMC needs SQMC, which is not built")
+    T = fk.T
+    if fk_info is None:
+        fk_info = fk.__class__(ssm=fk.ssm, data=fk.data[::-1])
+    pf = SMC(fk=fk, N=N, store_history=True)
+    tic = time.perf_counter()
+    pf.run()
+    h = pf.hist
+    ests = []
+    if method.startswith("FFBS"):
+        sub = method.split("_")[-1]
+        if sub == "ON2":
+            z = h.backward_sampling_ON2(N)
+        elif sub == "MCMC":
+            z = h.backward_sampling_mcmc(N)
+        elif sub == "hybrid":
+            z = h.backward_sampling_reject(N)
+        else:
+            z = h.backward_sampling_reject(N, max_trials=_PURE_REJECT_TRIALS)
+        for t in range(T - 1):
+            ests.append(as_device(add_func(t, z[t], z[t + 1])).mean())
+    else:
+        infopf = SMC(fk=fk_info, N=N, store_history=True)
+        infopf.run()
+        ih = infopf.hist
+        for t in range(T - 1):
+            psi = lambda x, xf, t=t: add_func(t, x, xf)          # noqa: E731
+            if method == "two-filter_ON2":
+                ests.append(h.two_filter_smoothing(t, infopf, psi, log_gamma))
+                continue
+            mf = mi = None
+            if method == "two-filter_ON_prop":
+                ti = T - 2 - t
+                a, b = _flat(ih.X[ti + 1]), _flat(h.X[t + 1])
+                mf = _norm_logpdf(_flat(h.X[t]), a.mean(), a.std(correction=0))
+                mi = _norm_logpdf(_flat(ih.X[ti]), b.mean(), b.std(correction=0))
+            ests.append(h.two_filter_smoothing(t, infopf, psi, log_gamma, linear_cost=True, modif_forward=mf,
+                                               modif_info=mi))
+    est = torch.stack([e.reshape(()) for e in ests]).cpu().numpy() if ests else np.zeros(0)
+    cpu_time = time.perf_counter() - tic
+    return {"est": est, "cpu": cpu_time}
