@@ -337,7 +337,9 @@ class Paris(OnlineSmootherMixin, Collector):
         for j in where.tolist():          # collectors.py:437-440
             lw = gp.lw + as_device(fk.logpt(g.t, gp.X, _repeat_rows(g.X[j // Np:j // Np + 1], N)))
             u = None if ue is None else float(ue[j])
-            B[j] = rs.multinomial_once(rs.exp_and_normalise(lw), u)
+            W = rs.exp_and_normalise(lw)
+            a = rs.multinomial_once(W, u)
+            B[j] = a if bool(W.sum() > 0) else 0      # no positive weight: 0, as the kernel's exact draw
         counts[0] = B.shape[0] - nrej
         counts[1] = nprops
 

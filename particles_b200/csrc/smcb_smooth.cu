@@ -108,7 +108,7 @@ __global__ void __launch_bounds__(kSmBlock) k_bs_on2(M m, smcb_smooth_desc d, Ph
             if (__syncthreads_and(!live || found >= 0)) break;
         }
         if (live) {
-            if (found < 0) found = last >= 0 ? last : N - 1;   // round-off: clip to the last positive weight
+            if (found < 0) found = last >= 0 ? last : 0;       // round-off / all-zero row (smcb_smooth.cuh)
             nxt = found;
             load_x<D>(d, t, nxt, xn);
             put_path<D>(d, t, j, nxt, xn);

@@ -6,6 +6,13 @@
 // d.X[t] and d.lw[t], the element strides d.x_stride_n / d.x_stride_c, the sizes d.N (particles at t), d.M (draws)
 // and d.max_trials, the CDF rows d.cdf + t * d.cdf_ld, and the injected proposals / log-uniforms d.prop / d.lu laid
 // out (t, M, max_trials).
+//
+// The rule every exact draw of a backward kernel follows (k_bs_on2, warp_exact_draw, and the plugin path of
+// smoothing.py / collectors.py): with v_n = lw_t[n] + logpt(t + 1, X_t[n], x) and e_n = exp(v_n - max v), the draw is
+// the first n with e_n > 0 and e_0 + ... + e_n >= u * sum e; a target above the re-summed total (round-off) gives the
+// last n with e_n > 0.  A row with no positive weight (every v_n is -inf) gives 0, as the reference's
+// searchsorted(cumsum(exp_and_normalise(v)), u) does on its all-NaN CDF.  A NaN v_n has weight zero here; in the
+// reference it makes the whole row NaN.
 #pragma once
 #include "smcb_common.cuh"
 #include "smcb_math.cuh"
@@ -122,8 +129,9 @@ __device__ int64_t warp_exact_draw(const M &m, const TransDensity<M> &td, const 
         if (pos) last = base + 31 - __clz(pos);
         c = __shfl_sync(kFull, cc, 31);
     }
-    // round-off: the target lies above the re-summed total -> the last particle of positive weight
-    return last >= 0 ? last : N - 1;
+    // round-off: the target lies above the re-summed total -> the last particle of positive weight (an all-zero row
+    // never gets here: its target is 0, which lane 0 meets at once)
+    return last >= 0 ? last : 0;
 }
 
 __device__ __forceinline__ long long warp_sum(long long v) {

@@ -391,6 +391,7 @@ class ParticleHistory(RollingParticleHistory):
         cdf = rs.cumsum(W)
         su = rs._uniforms(1, W) if u is None else torch.full((1,), float(u), dtype=torch.float64, device=W.device)
         _lib.check(ctx.lib.smcb_searchsorted(ctx.handle, ptr(cdf), W.shape[0], ptr(su), 1, C.c_void_p(out.data_ptr())))
+        out.masked_fill_(~(W.sum() > 0), 0)      # no positive weight (a NaN row): 0, as the kernels' exact draws
 
     def _plugin(self, method, M, idx, noise, nsteps, max_trials, bounds):
         """The reference's loops with ``fk.logpt`` on CUDA tensors (vectorised over M for MCMC / reject, over N per
