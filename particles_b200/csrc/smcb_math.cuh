@@ -176,8 +176,9 @@ __device__ __forceinline__ double texp_core(double x) {
     return __hiloint2double(__double2hiint(v) + ((k >> kExpTabBits) << 20), __double2loint(v));
 }
 // same with the power of two clamped to the normal range (two integer min / max instead of two fp64 selects):
-// the result SATURATES at ~2^-1022 / ~2^1024 instead of reaching 0 / +inf; +-inf and NaN give NaN.  For arguments
-// that are finite by construction (a model's exp of a finite state, a finite log-weight minus its maximum).
+// the result SATURATES at ~2^-1022 / ~2^1024 instead of reaching 0 / +inf; +-inf and a NaN with a zero low word give
+// NaN, a NaN with other payloads may give a finite value (see texp).  For arguments that are finite by construction (a
+// model's exp of a finite state, a finite log-weight minus its maximum).
 __device__ __forceinline__ double texp_sat(double x) {
     const double t = fma(x, kExpScaleT, kRintMagic);
     const double kd = t - kRintMagic;
@@ -195,11 +196,14 @@ __device__ __forceinline__ double texp_sat(double x) {
     return __hiloint2double(__double2hiint(v) + (q << 20), __double2loint(v));
 }
 
-// x <= ~709; 0 for x < -708 (incl. -inf), +inf for x > 709, NaN for NaN
+// x <= ~709; 0 for x < -708 (incl. -inf), +inf for x > 709, NaN for NaN of any payload.  texp_core adds the power of
+// two to the exponent field, so a NaN whose low word is all ones (0x7FFFFFFFFFFFFFFF) comes out of it as DBL_MAX (the
+// NaN an H100 makes of -inf - -inf has a zero low word, but a NaN may come from anywhere); the last select passes
+// x + inf instead, which is +inf above 709 and NaN for a NaN.
 __device__ __forceinline__ double texp(double x) {
     double res = texp_core(x);
     res = (x < -708.0) ? 0.0 : res;
-    res = (x > 709.0) ? CUDART_INF : res;
+    res = (x <= 709.0) ? res : x + CUDART_INF;
     return res;
 }
 // x <= 0 (weights relative to their maximum): no overflow select

@@ -231,6 +231,8 @@ __global__ void __launch_bounds__(kBatchBS) k_csmc(const smcb_csmc_desc d, const
                 double mxb[1] = {mloc};
                 block_max_all<1, BS>(mxb, s_red);        // its barriers also publish lwm
                 scan_range<BS>(LoadShiftedExp{lwm, mxb[0]}, 0, n, 0.0, CUDART_INF, cdf, s_warp);
+                // a row with no positive weight (every term -inf) gives 0, the rule of smcb_smooth.cuh: m = -inf makes
+                // every exp(v - m) texp(NaN) = NaN, so the key is NaN and the search stops at 0
                 idx = search_clamped(cdf, n, traj_uniform(key, t, udr) * cdf[n - 1]);
                 xnext = Xt[idx];
                 if (threadIdx.x == 0) traj[t] = xnext;

@@ -89,16 +89,22 @@ class StepReplay:
 
     # -------------------------------------------------------------- summaries
     def check_summary(self, s, X, lw, summ):
-        """Row s of the summary table (ESS, logLt, rs, log-mean) against the filter's log-weights of step s."""
-        m, S, Q, _ = lse_stats(lw)
-        lm = float(LD(m) + np.log(S / LD(self.N)))
-        ess = float(S * S / Q)
+        """Row s of the summary table (ESS, logLt, rs, log-mean) against the filter's log-weights of step s.  Weights
+        that are all -inf give NaN for all three, as NumPy does (and every later logLt is NaN)."""
+        with np.errstate(invalid="ignore"):
+            m, S, Q, _ = lse_stats(lw)
+            lm = float(LD(m) + np.log(S / LD(self.N)))
+            ess = float(S * S / Q)
         row = summ[s]
-        assert abs(row[3] - lm) <= 1e-12 * (1 + abs(lm)), f"step {s}: log-mean {row[3]!r} vs {lm!r}"
-        assert abs(row[0] - ess) <= 1e-12 * ess, f"step {s}: ESS {row[0]!r} vs {ess!r}"
+
+        def near(got, want, tol):
+            return (np.isnan(got) and np.isnan(want)) or abs(got - want) <= tol
+
+        assert near(row[3], lm, 1e-12 * (1 + abs(lm))), f"step {s}: log-mean {row[3]!r} vs {lm!r}"
+        assert near(row[0], ess, 1e-12 * ess), f"step {s}: ESS {row[0]!r} vs {ess!r}"
         loglt = lm if (s == 0 or row[2] != 0) else lm - summ[s - 1, 3]
         logLt = (0.0 if s == 0 else summ[s - 1, 1]) + loglt
-        assert abs(row[1] - logLt) <= 1e-12 * (1 + abs(logLt)), f"step {s}: logLt {row[1]!r} vs {logLt!r}"
+        assert near(row[1], logLt, 1e-12 * (1 + abs(logLt))), f"step {s}: logLt {row[1]!r} vs {logLt!r}"
         return lm, ess
 
     # ---------------------------------------------------------------- step 0

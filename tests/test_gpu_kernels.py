@@ -96,6 +96,17 @@ def test_device_math(pb):
     e = run(4, x)
     np.testing.assert_allclose(e[ok], ref[ok], rtol=4.5e-16)
     assert np.all(e[~ok] == 0.0) and np.isnan(run(4, np.array([np.nan, 1.0]))[0])
+    # NaN with any payload, among them low words of all ones (texp adds to the exponent field of its core's result),
+    # and the NaN the device itself makes of -inf - -inf
+    nans = np.array([0x7FF8000000000000, 0x7FFFFFFFFFFFFFFF, 0xFFFFFFFFFFFFFFFF, 0x7FF0000000000001,
+                     0x7FF80000FFFFFFFF], dtype=np.uint64).view(np.float64)
+    for fn in (0, 4):
+        assert np.isnan(run(fn, nans)).all(), (fn, run(fn, nans))
+    made = dev(np.full(4, -np.inf))
+    made = made - made                                                  # NaN made by the device
+    out = empty(4)
+    _lib.check(ctx.lib.smcb_device_math(ctx.handle, 4, ptr(made), ptr(out), 4))
+    assert np.isnan(host(out)).all(), host(made).view(np.uint64)
     assert run(4, np.array([710.0, 1.0]))[0] == np.inf
     np.testing.assert_allclose(run(5, u), np.log(u), rtol=7e-16, atol=3e-19)
     np.testing.assert_allclose(run(6, v), np.sin(2 * np.pi * v), atol=2e-15, rtol=0)
