@@ -60,13 +60,14 @@ int smcb_weights_from_stats(smcb_ctx *ctx, const double *lw, int64_t n, const do
 #define SMCB_LSE_SUM 0  /* log_sum_exp   resampling.py:247-270            */
 #define SMCB_LSE_MEAN 1 /* log_mean_exp  resampling.py:291-317 (W optional) */
 #define SMCB_LSE_ESSL 2 /* essl          resampling.py:166-188            */
+/* every mode gives NaN when v holds a NaN or a +inf, or is -inf throughout, as the reference does */
 int smcb_lse(smcb_ctx *ctx, int mode, const double *v, const double *W, int64_t n,
              double *out);
 
 /* exp_and_normalise, resampling.py:138-163 */
 int smcb_exp_and_normalise(smcb_ctx *ctx, const double *lw, int64_t n, double *W_out);
 
-/* wmean_and_var, resampling.py:320-338; x is SoA (d, n); out = {mean[d], var[d]} */
+/* wmean_and_var, resampling.py:320-338; x is SoA (d, n) with 1 <= d <= 32; out = {mean[d], var[d]} */
 int smcb_wmean_and_var(smcb_ctx *ctx, const double *W, const double *x, int64_t n, int d,
                        double *out);
 

@@ -103,6 +103,9 @@ enum { kModeNormalise = 10, kModeWeightedMean = 11 };
 
 // one pass: (max, sum exp, sum exp^2) of v, deterministic grid merge, scalars out.
 // mode kModeNormalise also rewrites NaN -> -inf in place (resampling.py:220).
+// The other modes follow the reference's m + log(sum(exp(v - m))) at the edges: a NaN anywhere, a +inf anywhere or
+// every entry -inf gives NaN (NaN - m, inf - inf, -inf - -inf).  A NaN marks its accumulator's max as well as its sum,
+// so that no merge drops it as an empty (max -inf) partial.
 template <int MODE>
 __global__ void __launch_bounds__(kBlock) k_lse(double *v, const double *__restrict__ W, int64_t n,
                                                double *partials, unsigned int *ticket,
@@ -140,14 +143,14 @@ __global__ void __launch_bounds__(kBlock) k_lse(double *v, const double *__restr
             }
             lse3_add_batch_f<1>(acc[0], x);
         }
-        if (saw_nan) acc[0].s = CUDART_NAN;
+        if (saw_nan) { acc[0].m = CUDART_NAN; acc[0].s = CUDART_NAN; }
     } else {
         for (; i < n; i += stride) {
             double x = v[i];
             // log_mean_exp(v, W): m + log( sum W e^{v-m} / sum W )  (resampling.py:312-317)
             double w = W[i];
             sw += w;
-            if (x != x) { acc[0].s = CUDART_NAN; continue; }
+            if (x != x) { acc[0].m = CUDART_NAN; acc[0].s = CUDART_NAN; continue; }
             if (x == -CUDART_INF) continue;
             double d = x - acc[0].m;
             double e = exp(-fabs(d));
@@ -179,22 +182,23 @@ __global__ void __launch_bounds__(kBlock) k_lse(double *v, const double *__restr
             s_tot = t;
         }
         __syncthreads();
-        if (threadIdx.x == 0) out[0] = tot[0].m + log(tot[0].s / s_tot);
+        if (threadIdx.x == 0) out[0] = (fabs(tot[0].m) == CUDART_INF) ? CUDART_NAN : tot[0].m + log(tot[0].s / s_tot);
         return;
     }
     if (threadIdx.x != 0) return;
     const Lse3 t = tot[0];
+    const bool edge = (fabs(t.m) == CUDART_INF);             // all -inf, or a +inf: NaN, as NumPy gives
     if (MODE == kModeNormalise) {
         double lm, ess;
         weights_scalars(t, (double)n, lm, ess);
         out[0] = t.m; out[1] = lm; out[2] = ess;
         out[3] = (lm != lm) ? CUDART_NAN : t.s;
     } else if (MODE == SMCB_LSE_SUM) {
-        out[0] = t.m + log(t.s);
+        out[0] = edge ? CUDART_NAN : t.m + log(t.s);
     } else if (MODE == SMCB_LSE_MEAN) {
-        out[0] = t.m + log(t.s / (double)n);
+        out[0] = edge ? CUDART_NAN : t.m + log(t.s / (double)n);
     } else if (MODE == SMCB_LSE_ESSL) {
-        out[0] = (t.s * t.s) / t.q;
+        out[0] = edge ? CUDART_NAN : (t.s * t.s) / t.q;
     }
 }
 
@@ -274,7 +278,7 @@ __global__ void __launch_bounds__(kBlock) k_max_sum(const double *__restrict__ v
     const int64_t stride = (int64_t)gridDim.x * kBlock;
     for (int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x; i < n; i += stride) {
         double x = v[i];
-        if (x != x) acc[0].s = CUDART_NAN;
+        if (x != x) { acc[0].m = CUDART_NAN; acc[0].s = CUDART_NAN; continue; }     // kept through every merge
         lse3_add(acc[0], x);
     }
     Lse3 tot[1];
@@ -383,7 +387,9 @@ __global__ void __launch_bounds__(kBlock) k_wmoments(const double *__restrict__ 
 extern "C" int smcb_wmean_and_var(smcb_ctx *c, const double *W, const double *x, int64_t n, int d,
                                   double *out) {
     SMCB_REQUIRE(c && W && x && out, "smcb_wmean_and_var: NULL argument");
-    SMCB_REQUIRE(n >= 1 && d >= 1 && d <= 16, "smcb_wmean_and_var: need n >= 1, 1 <= d <= 16");
+    // d <= 32, the samplers' largest dimension: (592 + 1) (2 d + 1) partials fit kWsPartials, 2 d + 1 <= kBlock
+    SMCB_REQUIRE(n >= 1 && d >= 1 && d <= 32, "smcb_wmean_and_var: need n >= 1, 1 <= d <= 32 (got n=%lld d=%d)",
+                 (long long)n, d);
     int grid = grid_for(n, kBlock * 4);
     if (grid > 592) grid = 592;
     LAUNCH(c, k_wmoments, grid, kBlock, W, x, n, d, c->ws, c->counters + 1, out);
@@ -932,12 +938,15 @@ __global__ void __launch_bounds__(kBlock) k_logpdf1(int kind, const double *__re
             const double z = (xv - a) / b;
             r = c0 - 0.5 * (p0 + 1.0) * log1p(z * z / p0) - log(b);
         } else if (kind == 1) {           // a = rate b (array or scalar); c0 = -gammaln(a_shape)
-            r = (xv > 0.0) ? p0 * log(a) + c0 + (p0 - 1.0) * log(xv) - a * xv : -CUDART_INF;
+            // scipy's xlogy(a - 1, x): the term is 0 when a == 1, also at x = 0 and x = +inf; at x = 0 it is +inf for
+            // a < 1 and -inf for a > 1, and x = +inf gives -inf for a <= 1 and NaN (inf - inf) for a > 1
+            const double xl = (p0 == 1.0) ? 0.0 : (p0 - 1.0) * log(xv);
+            r = (xv != xv) ? xv : (xv >= 0.0) ? p0 * log(a) + c0 + xl - a * xv : -CUDART_INF;
         } else if (kind == 2) {
             r = -log(2.0 * b) - fabs(xv - a) / b;
-        } else {
-            const double z = (xv - a) / b;
-            r = -z - 2.0 * log1p(exp(-z)) - log(b);
+        } else {                          // scipy's symmetric form: exp(-|z|) cannot overflow
+            const double y = -fabs((xv - a) / b);
+            r = y - 2.0 * log1p(exp(y)) - log(b);
         }
         out[i] = r;
     }

@@ -116,11 +116,27 @@ __device__ __forceinline__ void scan_chunks(const LOAD &load, int64_t n, int til
         const T up = __shfl_up_sync(0xffffffffu, iw, 1);
         const T excl = (lane == 0) ? woff : (woff + up);
         const int b = (int)blockIdx.x;
-        if (b == 0 && tid == 0) s_pref[0] = (T)0;
+        // the base of chunk b is the LARGEST inclusive prefix of chunks 0..b-1, not the prefix of chunk b - 1 alone:
+        // excl + c[j] rounds differently on either side of a thread boundary, so after a chunk that sums to 0 the
+        // prefix of chunk b - 1 can fall below that of chunk b - 2 -- and below what CTA b - 1 clamped its last
+        // value to.  The max is exact, so CTA b's base is bit for bit CTA b - 1's upper clamp p_next.
+        __shared__ T s_max[kBlock / 32];
+        T pm = (T)0;
 #pragma unroll
-        for (int j = 0; j < 4; j++) {
-            if (4 * tid + j + 1 == b) s_pref[0] = excl + c[j];           // inclusive prefix of chunk b - 1
+        for (int j = 0; j < 4; j++)
+            if (4 * tid + j < b) pm = tmax(pm, excl + c[j]);
+#pragma unroll
+        for (int d = 16; d > 0; d >>= 1) pm = tmax(pm, __shfl_xor_sync(0xffffffffu, pm, d));
+        if (lane == 0) s_max[warp] = pm;
+#pragma unroll
+        for (int j = 0; j < 4; j++)
             if (4 * tid + j == b) s_pref[1] = excl + c[j];               // inclusive prefix of chunk b
+        __syncthreads();
+        if (tid == 0) {
+            T m = s_max[0];
+#pragma unroll
+            for (int w = 1; w < kBlock / 32; w++) m = tmax(m, s_max[w]);
+            s_pref[0] = m;
         }
         __syncthreads();
     }
