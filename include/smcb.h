@@ -650,6 +650,46 @@ int smcb_csmc_plan(smcb_ctx *ctx, const smcb_csmc_desc *desc, int64_t out[2]);
 /* the forward pass and the trajectory draw of every chain: one launch on the context's stream, no host sync */
 int smcb_csmc_run(smcb_ctx *ctx, const smcb_csmc_desc *desc);
 
+/* ---------------------------------------------------------------------------
+ * hidden Markov models (particles/hmm.py, BaumWelch): B finite-state HMMs with K <= SMCB_HMM_MAX_K states.
+ * Per-HMM arrays are time-major rows of a buffer of `ld` rows: element (b, t, k) of pred / filt / logft / smth is
+ * at [(b * ld + t) * K + k], logpyt (b, t) at [b * ld + t].  trans (b) is at trans + b * trans_stride (K x K, row
+ * j = from-state), init (b) at init + b * init_stride; a stride of 0 shares one matrix / vector across the batch.
+ * K <= 32 runs one warp per HMM, 33 <= K <= 128 one CTA per HMM; every sum over states is a fixed tree (warps: xor
+ * butterfly; across warps: in warp order), so the bits depend on the inputs only.
+ * ------------------------------------------------------------------------- */
+#define SMCB_HMM_MAX_K 128
+#define SMCB_HMM_FORWARD 0  /* rows [t0, t1): pred_t = filt_{t-1} P (sum in j order; init at t = 0),
+                               lp = log pred_t + logft_t, logpyt_t = LSE(lp), filt_t = exp(lp - logpyt_t)       */
+#define SMCB_HMM_BACKWARD 1 /* rows [0, t1): ctg_k <- LSE_j(log P_kj + logft_{t+1,j} + ctg_j),
+                               smth_t = exp_and_normalise(log filt_t + ctg), smth_{t1-1} = filt_{t1-1}         */
+#define SMCB_HMM_SAMPLE 2   /* rows t1-2 .. 0 of N trajectories per HMM, given paths row t1-1: per t the K column
+                               CDFs C[j][k] = cumsum_k exp_and_normalise_k(log P_kj + log filt_t,k), the draw
+                               #{k : C[path_{t+1}][k] < u}, clipped to K - 1; u = U[(b, t, n)] if U, else
+                               Philox(seed; n, t, b) under its own purpose                                   */
+
+typedef struct {
+    int32_t method, K;
+    int64_t B;                 /* HMMs                                                                     */
+    int64_t ld;                /* rows per HMM in the time-major buffers                                   */
+    int64_t t0, t1;            /* FORWARD: rows [t0, t1); BACKWARD / SAMPLE: t1 = T rows filled            */
+    int64_t N;                 /* SAMPLE: trajectories per HMM                                             */
+    uint64_t seed;             /* SAMPLE: Philox key when U is NULL                                        */
+    const double *trans;       /* (K, K) per HMM                                                           */
+    int64_t trans_stride;
+    const double *init;        /* (K) per HMM                                                              */
+    int64_t init_stride;
+    const double *logft;       /* (B, ld, K) log-density of y_t given x_t = k                              */
+    double *pred, *filt;       /* (B, ld, K) FORWARD out; filt read by BACKWARD / SAMPLE                   */
+    double *logpyt;            /* (B, ld) FORWARD out                                                      */
+    double *smth;              /* (B, ld, K) BACKWARD out                                                  */
+    const double *U;           /* SAMPLE: NULL, or (B, t1 - 1, N) injected uniforms                        */
+    int64_t *paths;            /* SAMPLE: (B, t1, N); row t1 - 1 is read, rows t1 - 2 .. 0 written         */
+} smcb_hmm_desc;
+
+/* one kernel launch on the context's stream, no host sync; K > SMCB_HMM_MAX_K -> SMCB_ENOSYS */
+int smcb_hmm(smcb_ctx *ctx, const smcb_hmm_desc *desc);
+
 #ifdef __cplusplus
 }
 #endif

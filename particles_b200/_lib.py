@@ -141,6 +141,20 @@ class CsmcDesc(C.Structure):
     ]
 
 
+HMM_FORWARD, HMM_BACKWARD, HMM_SAMPLE = 0, 1, 2
+HMM_MAX_K = 128
+
+
+class HmmDesc(C.Structure):
+    _fields_ = [
+        ("method", C.c_int32), ("K", C.c_int32), ("B", C.c_int64), ("ld", C.c_int64),
+        ("t0", C.c_int64), ("t1", C.c_int64), ("N", C.c_int64), ("seed", C.c_uint64),
+        ("trans", c_dp), ("trans_stride", C.c_int64), ("init", c_dp), ("init_stride", C.c_int64),
+        ("logft", c_dp), ("pred", c_dp), ("filt", c_dp), ("logpyt", c_dp), ("smth", c_dp),
+        ("U", c_dp), ("paths", c_dp),
+    ]
+
+
 class VsDesc(C.Structure):
     _fields_ = [
         ("p", C.c_int32), ("use_ldet", C.c_int32), ("xtx", c_dp), ("xty", c_dp), ("vm2", C.c_double),
@@ -236,6 +250,7 @@ PROTOTYPES = {
                                        c_dp, c_dp, c_dp, c_dp]),
     "smcb_csmc_plan": (C.c_int, [C.c_void_p, C.POINTER(CsmcDesc), C.POINTER(C.c_int64)]),
     "smcb_csmc_run": (C.c_int, [C.c_void_p, C.POINTER(CsmcDesc)]),
+    "smcb_hmm": (C.c_int, [C.c_void_p, C.POINTER(HmmDesc)]),
 }
 
 _lib = None
