@@ -690,6 +690,41 @@ typedef struct {
 /* one kernel launch on the context's stream, no host sync; K > SMCB_HMM_MAX_K -> SMCB_ENOSYS */
 int smcb_hmm(smcb_ctx *ctx, const smcb_hmm_desc *desc);
 
+/* ---------------------------------------------------------------------------
+ * Kalman filter and RTS smoother (particles/kalman.py, Kalman): B linear-Gaussian models X_t = F X_{t-1} + U,
+ * Y_t = G X_t + V with dx, dy <= SMCB_KALMAN_MAX_D.  Per-model arrays are time-major rows of a buffer of `ld` rows:
+ * mean (b, t, i) at [(b * ld + t) * dx + i], cov (b, t, i, j) at [((b * ld + t) * dx + i) * dx + j], logpyt (b, t)
+ * at [b * ld + t]; observation (b, t, i) at y[b * y_stride + t * dy + i].  Parameter (b) is at p + b * p_stride
+ * (F, covX, cov0: dx x dx; G: dy x dx; covY: dy x dy; mu0: dx, all row-major); a stride of 0 shares it.
+ * dx = dy = 1 runs one thread per model, otherwise one warp per model; every sum runs in index order, so the bits
+ * depend on the inputs only.  A non-positive Cholesky pivot (S or P_{t+1} not positive definite) gives NaN, which
+ * fills that model's rows from that step on.
+ * ------------------------------------------------------------------------- */
+#define SMCB_KALMAN_MAX_D 32
+#define SMCB_KALMAN_FILTER 0 /* rows [t0, t1): pred = (mu0, cov0) at t = 0, else (F m, (F Sig) F' + covX);
+                                S = (G P) G' + covY, K = P G' S^-1 through chol(S), filt = (m + K r, P - (K G) P),
+                                logpyt: N(G pm, S) log-density of y_t                                           */
+#define SMCB_KALMAN_SMOOTH 1 /* rows [0, t1): J = Sig_f F' P_{t+1}^-1 through chol(P_{t+1}),
+                                smth = (m_f + J (m_s' - m_{t+1}), Sig_f + (J (Sig_s' - P_{t+1})) J'),
+                                smth_{t1-1} = filt_{t1-1}                                                       */
+
+typedef struct {
+    int32_t method, dx, dy, pad_;
+    int64_t B;                 /* models                                                                   */
+    int64_t ld;                /* rows per model in the time-major buffers                                 */
+    int64_t t0, t1;            /* FILTER: rows [t0, t1); SMOOTH: t1 = T rows filtered                      */
+    const double *F, *G, *covX, *covY, *mu0, *cov0;
+    int64_t F_stride, G_stride, covX_stride, covY_stride, mu0_stride, cov0_stride;
+    const double *y;           /* FILTER: observations                                                     */
+    int64_t y_stride;
+    double *pred_mean, *pred_cov, *filt_mean, *filt_cov;   /* FILTER out; read by SMOOTH                   */
+    double *logpyt;            /* FILTER out                                                               */
+    double *smth_mean, *smth_cov;                          /* SMOOTH out                                   */
+} smcb_kalman_desc;
+
+/* one kernel launch on the context's stream, no host sync; dx or dy > SMCB_KALMAN_MAX_D -> SMCB_ENOSYS */
+int smcb_kalman(smcb_ctx *ctx, const smcb_kalman_desc *desc);
+
 #ifdef __cplusplus
 }
 #endif

@@ -8,6 +8,7 @@ from .core import SMC, FeynmanKac, multiSMC  # noqa: F401
 from .device import seed  # noqa: F401
 from . import hmm  # noqa: F401
 from .hmm import HMM, GaussianHMM, BaumWelch  # noqa: F401
+from . import kalman  # noqa: F401
 
 __version__ = "0.1.0"
 

@@ -155,6 +155,22 @@ class HmmDesc(C.Structure):
     ]
 
 
+KALMAN_FILTER, KALMAN_SMOOTH = 0, 1
+KALMAN_MAX_D = 32
+
+
+class KalmanDesc(C.Structure):
+    _fields_ = [
+        ("method", C.c_int32), ("dx", C.c_int32), ("dy", C.c_int32), ("pad_", C.c_int32),
+        ("B", C.c_int64), ("ld", C.c_int64), ("t0", C.c_int64), ("t1", C.c_int64),
+        ("F", c_dp), ("G", c_dp), ("covX", c_dp), ("covY", c_dp), ("mu0", c_dp), ("cov0", c_dp),
+        ("F_stride", C.c_int64), ("G_stride", C.c_int64), ("covX_stride", C.c_int64), ("covY_stride", C.c_int64),
+        ("mu0_stride", C.c_int64), ("cov0_stride", C.c_int64), ("y", c_dp), ("y_stride", C.c_int64),
+        ("pred_mean", c_dp), ("pred_cov", c_dp), ("filt_mean", c_dp), ("filt_cov", c_dp), ("logpyt", c_dp),
+        ("smth_mean", c_dp), ("smth_cov", c_dp),
+    ]
+
+
 class VsDesc(C.Structure):
     _fields_ = [
         ("p", C.c_int32), ("use_ldet", C.c_int32), ("xtx", c_dp), ("xty", c_dp), ("vm2", C.c_double),
@@ -251,6 +267,7 @@ PROTOTYPES = {
     "smcb_csmc_plan": (C.c_int, [C.c_void_p, C.POINTER(CsmcDesc), C.POINTER(C.c_int64)]),
     "smcb_csmc_run": (C.c_int, [C.c_void_p, C.POINTER(CsmcDesc)]),
     "smcb_hmm": (C.c_int, [C.c_void_p, C.POINTER(HmmDesc)]),
+    "smcb_kalman": (C.c_int, [C.c_void_p, C.POINTER(KalmanDesc)]),
 }
 
 _lib = None

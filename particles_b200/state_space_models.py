@@ -438,6 +438,8 @@ def fused_spec(fk, smoothing_hooks=False):
     make = _SPECS.get(ssm_cls.__name__)
     if make is None:
         return None
+    if getattr(ssm, "batch", None) is not None:
+        raise ValueError(f"fused_spec: a batch of B = {ssm.batch} {ssm_cls.__name__} models runs in kalman.Kalman only")
     spec = make(ssm, fk.T, fk.data) if make in (spec_mvlingauss, spec_discretecox) else make(ssm, fk.T)
     if spec is None:
         return None
