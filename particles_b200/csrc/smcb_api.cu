@@ -40,8 +40,8 @@ extern "C" int smcb_create(smcb_ctx **out, int device, uint64_t seed) {
     c->launches = 0;
     c->ws_bytes = kWsBytes;
     SMCB_CUDA(cudaMalloc(&c->ws, c->ws_bytes));
-    SMCB_CUDA(cudaMalloc(&c->counters, 64 * sizeof(unsigned int)));
-    SMCB_CUDA(cudaMemset(c->counters, 0, 64 * sizeof(unsigned int)));
+    SMCB_CUDA(cudaMalloc(&c->counters, kTicketSlots * sizeof(unsigned int)));
+    SMCB_CUDA(cudaMemset(c->counters, 0, kTicketSlots * sizeof(unsigned int)));
     {   // lookup tables of the step kernels' elementary functions (long double on the host, once)
         double *h = new (std::nothrow) double[kMathTabDoubles];
         SMCB_REQUIRE(h != nullptr, "smcb_create: out of host memory");
@@ -79,13 +79,6 @@ extern "C" int smcb_seed(smcb_ctx *c, uint64_t seed) {
 }
 
 extern "C" int64_t smcb_launch_count(const smcb_ctx *c) { return c ? c->launches : 0; }
-
-#define LAUNCH(ctx, kern, grid, block, ...)                                      \
-    do {                                                                         \
-        kern<<<(grid), (block), 0, (ctx)->stream>>>(__VA_ARGS__);                \
-        (ctx)->launches++;                                                       \
-        SMCB_CUDA(cudaGetLastError());                                           \
-    } while (0)
 
 static int check_ws(smcb_ctx *c, size_t need) {
     if (need <= c->ws_bytes) return SMCB_OK;
@@ -161,8 +154,7 @@ __global__ void __launch_bounds__(kBlock) k_lse(double *v, const double *__restr
     if (MODE == kModeWeightedMean) {
         // carry sum W in the q slot; it must NOT be rescaled by the merges, so reduce it apart
         __shared__ double s_sw[kBlock / 32];
-#pragma unroll
-        for (int mask = 16; mask > 0; mask >>= 1) sw += __shfl_xor_sync(0xffffffffu, sw, mask);
+        sw = warp_sum(sw);
         if ((threadIdx.x & 31) == 0) s_sw[threadIdx.x >> 5] = sw;
         __syncthreads();
         if (threadIdx.x == 0) {
@@ -234,9 +226,10 @@ extern "C" int smcb_normalise(smcb_ctx *c, double *lw, int64_t n, double *W_out,
     SMCB_REQUIRE(c && lw && stats_out, "smcb_normalise: NULL argument");
     SMCB_REQUIRE(n >= 1, "smcb_normalise: n must be >= 1 (got %lld)", (long long)n);
     const int grid = grid_for(n, kBlock * 4);
-    LAUNCH(c, k_lse<kModeNormalise>, grid, kBlock, lw, nullptr, n, c->ws, c->counters + 0, stats_out);
-    if (W_out) LAUNCH(c, k_exp_normalise, grid_for(n, kBlock * 4), kBlock, lw, n, stats_out, W_out);
-    return SMCB_OK;
+    SMCB_TRY(launch(c, k_lse<kModeNormalise>, grid, kBlock, 0, lw, nullptr, n, c->ws, c->counters + kTicketLse,
+                    stats_out));
+    if (!W_out) return SMCB_OK;
+    return launch(c, k_exp_normalise, grid_for(n, kBlock * 4), kBlock, 0, lw, n, stats_out, W_out);
 }
 
 // W = exp(lw - m) / s from statistics the caller already holds (stats = {m, ., ., s}: the layout smcb_normalise
@@ -244,8 +237,7 @@ extern "C" int smcb_normalise(smcb_ctx *c, double *lw, int64_t n, double *W_out,
 extern "C" int smcb_weights_from_stats(smcb_ctx *c, const double *lw, int64_t n, const double *stats, double *W_out) {
     SMCB_REQUIRE(c && lw && stats && W_out, "smcb_weights_from_stats: NULL argument");
     SMCB_REQUIRE(n >= 1, "smcb_weights_from_stats: n must be >= 1");
-    LAUNCH(c, k_exp_normalise, grid_for(n, kBlock * 4), kBlock, lw, n, stats, W_out);
-    return SMCB_OK;
+    return launch(c, k_exp_normalise, grid_for(n, kBlock * 4), kBlock, 0, lw, n, stats, W_out);
 }
 
 extern "C" int smcb_lse(smcb_ctx *c, int mode, const double *v, const double *W, int64_t n,
@@ -254,19 +246,15 @@ extern "C" int smcb_lse(smcb_ctx *c, int mode, const double *v, const double *W,
     SMCB_REQUIRE(n >= 1, "smcb_lse: n must be >= 1");
     const int grid = grid_for(n, kBlock * 4);
     double *vv = const_cast<double *>(v);
-    if (mode == SMCB_LSE_SUM) {
-        LAUNCH(c, k_lse<SMCB_LSE_SUM>, grid, kBlock, vv, nullptr, n, c->ws, c->counters + 0, out);
-    } else if (mode == SMCB_LSE_MEAN && W == nullptr) {
-        LAUNCH(c, k_lse<SMCB_LSE_MEAN>, grid, kBlock, vv, nullptr, n, c->ws, c->counters + 0, out);
-    } else if (mode == SMCB_LSE_MEAN) {
-        LAUNCH(c, k_lse<kModeWeightedMean>, grid, kBlock, vv, W, n, c->ws, c->counters + 0, out);
-    } else if (mode == SMCB_LSE_ESSL) {
-        LAUNCH(c, k_lse<SMCB_LSE_ESSL>, grid, kBlock, vv, nullptr, n, c->ws, c->counters + 0, out);
-    } else {
-        set_error("smcb_lse: unknown mode %d", mode);
-        return SMCB_EINVAL;
-    }
-    return SMCB_OK;
+    unsigned int *ticket = c->counters + kTicketLse;
+    if (mode == SMCB_LSE_SUM) return launch(c, k_lse<SMCB_LSE_SUM>, grid, kBlock, 0, vv, nullptr, n, c->ws, ticket, out);
+    if (mode == SMCB_LSE_MEAN && W == nullptr)
+        return launch(c, k_lse<SMCB_LSE_MEAN>, grid, kBlock, 0, vv, nullptr, n, c->ws, ticket, out);
+    if (mode == SMCB_LSE_MEAN) return launch(c, k_lse<kModeWeightedMean>, grid, kBlock, 0, vv, W, n, c->ws, ticket, out);
+    if (mode == SMCB_LSE_ESSL)
+        return launch(c, k_lse<SMCB_LSE_ESSL>, grid, kBlock, 0, vv, nullptr, n, c->ws, ticket, out);
+    set_error("smcb_lse: unknown mode %d", mode);
+    return SMCB_EINVAL;
 }
 
 // exp_and_normalise: m = max, w = exp(lw - m), W = w / sum(w)  (no NaN rewrite)
@@ -294,9 +282,8 @@ extern "C" int smcb_exp_and_normalise(smcb_ctx *c, const double *lw, int64_t n, 
     SMCB_REQUIRE(c && lw && W_out, "smcb_exp_and_normalise: NULL argument");
     SMCB_REQUIRE(n >= 1, "smcb_exp_and_normalise: n must be >= 1");
     double *stats = c->ws + kWsPartials;  // 4 doubles right after the partials
-    LAUNCH(c, k_max_sum, grid_for(n, kBlock * 4), kBlock, lw, n, c->ws, c->counters + 0, stats);
-    LAUNCH(c, k_exp_normalise, grid_for(n, kBlock * 4), kBlock, lw, n, stats, W_out);
-    return SMCB_OK;
+    SMCB_TRY(launch(c, k_max_sum, grid_for(n, kBlock * 4), kBlock, 0, lw, n, c->ws, c->counters + kTicketLse, stats));
+    return launch(c, k_exp_normalise, grid_for(n, kBlock * 4), kBlock, 0, lw, n, stats, W_out);
 }
 
 // wmean_and_var (resampling.py:320-338): np.average(x, weights=W), np.average(x^2, weights=W)
@@ -307,7 +294,6 @@ __global__ void __launch_bounds__(kBlock) k_wmoments(const double *__restrict__ 
                                                     double *out) {
     // partials layout: [block][3*d + 1]: sum W, then per component sum W x, sum W x^2
     __shared__ double s_red[9][kBlock / 32];
-    __shared__ bool s_last;
     const int nv = 1 + 2 * d;
     const int64_t stride = (int64_t)gridDim.x * kBlock;
     // ONE pass over W and x per chunk of 4 components (d <= 4: one pass in all; the first version re-read W for every
@@ -345,9 +331,7 @@ __global__ void __launch_bounds__(kBlock) k_wmoments(const double *__restrict__ 
         }
 #pragma unroll
         for (int q = 0; q < 9; q++) {
-            double acc = a[q];
-#pragma unroll
-            for (int mask = 16; mask > 0; mask >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, mask);
+            const double acc = warp_sum(a[q]);
             if ((threadIdx.x & 31) == 0) s_red[q][threadIdx.x >> 5] = acc;
         }
         __syncthreads();
@@ -360,13 +344,7 @@ __global__ void __launch_bounds__(kBlock) k_wmoments(const double *__restrict__ 
         }
         __syncthreads();
     }
-    if (threadIdx.x == 0) {
-        __threadfence();
-        s_last = (atomicInc(ticket, gridDim.x - 1) == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
+    if (!last_block(ticket)) return;
     if (threadIdx.x < nv) {
         double t = 0.0;
         for (int k = 0; k < (int)gridDim.x; k++)
@@ -392,8 +370,7 @@ extern "C" int smcb_wmean_and_var(smcb_ctx *c, const double *W, const double *x,
                  (long long)n, d);
     int grid = grid_for(n, kBlock * 4);
     if (grid > 592) grid = 592;
-    LAUNCH(c, k_wmoments, grid, kBlock, W, x, n, d, c->ws, c->counters + 1, out);
-    return SMCB_OK;
+    return launch(c, k_wmoments, grid, kBlock, 0, W, x, n, d, c->ws, c->counters + kTicketWmoments, out);
 }
 
 // ---------------------------------------------------------------------------
@@ -481,11 +458,8 @@ static int run_scan(smcb_ctx *c, const LOAD &load, int64_t n, T *out, int slot =
     const int tpc = (int)((tiles + want - 1) / want);
     const int nchunks = (int)((tiles + tpc - 1) / tpc);
     T *sums = reinterpret_cast<T *>(st.chunk_sum);
-    k_scan_sums<T, LOAD><<<nchunks, kBlock, 0, c->stream>>>(load, n, tpc, sums);
-    k_scan_chunks<T, LOAD><<<nchunks, kBlock, 0, c->stream>>>(load, n, tpc, sums, nchunks, out);
-    c->launches += 2;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    SMCB_TRY(launch(c, k_scan_sums<T, LOAD>, nchunks, kBlock, 0, load, n, tpc, sums));
+    return launch(c, k_scan_chunks<T, LOAD>, nchunks, kBlock, 0, load, n, tpc, sums, nchunks, out);
 }
 
 extern "C" int smcb_cumsum(smcb_ctx *c, const double *w, int64_t n, double *cdf_out) {
@@ -582,7 +556,8 @@ static int run_search(smcb_ctx *c, const double *cdf, int64_t n, const SU &su, i
     int rc = check_ws(c, base + 2 * (need > sc ? need : sc) + 64);
     if (rc) return rc;
     int64_t *bnd = reinterpret_cast<int64_t *>((char *)c->ws + base);
-    k_search_bounds<SU><<<(int)((tiles + 1 + kBlock - 1) / kBlock), kBlock, 0, c->stream>>>(cdf, n, su, m, tiles, bnd);
+    SMCB_TRY(launch(c, k_search_bounds<SU>, (int)((tiles + 1 + kBlock - 1) / kBlock), kBlock, 0, cdf, n, su, m, tiles,
+                    bnd));
     static int occ = 0;                        // resident CTAs per SM of this instantiation: the grid is ONE full wave
     if (occ == 0) {
         int o = 0;
@@ -591,10 +566,7 @@ static int run_search(smcb_ctx *c, const double *cdf, int64_t n, const SU &su, i
     }
     const int64_t wave = (int64_t)kSMs * occ;
     int grid = (int)(tiles < wave ? tiles : wave);
-    k_search<SU><<<grid, kBlock, 0, c->stream>>>(cdf, n, su, m, A, a_offset, bnd);
-    c->launches += 2;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    return launch(c, k_search<SU>, grid, kBlock, 0, cdf, n, su, m, A, a_offset, bnd);
 }
 
 extern "C" int smcb_searchsorted(smcb_ctx *c, const double *cdf, int64_t n, const double *su,
@@ -634,14 +606,14 @@ __global__ void __launch_bounds__(kBlock) k_std_normal(Philox key, uint64_t call
 extern "C" int smcb_uniform(smcb_ctx *c, double *out, int64_t n) {
     SMCB_REQUIRE(c && out && n >= 0, "smcb_uniform: bad argument");
     if (n == 0) return SMCB_OK;
-    LAUNCH(c, k_uniform, grid_for((n + 1) / 2, kBlock * 4), kBlock, key_of(c->seed), c->api_counter++, out, n);
-    return SMCB_OK;
+    return launch(c, k_uniform, grid_for((n + 1) / 2, kBlock * 4), kBlock, 0, key_of(c->seed), c->api_counter++, out,
+                  n);
 }
 extern "C" int smcb_standard_normal(smcb_ctx *c, double *out, int64_t n) {
     SMCB_REQUIRE(c && out && n >= 0, "smcb_standard_normal: bad argument");
     if (n == 0) return SMCB_OK;
-    LAUNCH(c, k_std_normal, grid_for((n + 1) / 2, kBlock * 4), kBlock, key_of(c->seed), c->api_counter++, out, n);
-    return SMCB_OK;
+    return launch(c, k_std_normal, grid_for((n + 1) / 2, kBlock * 4), kBlock, 0, key_of(c->seed), c->api_counter++,
+                  out, n);
 }
 
 // residual resampling, deterministic part (resampling.py:622):
@@ -777,9 +749,7 @@ extern "C" int smcb_resample(smcb_ctx *c, int scheme, const double *W, int64_t n
             if (n > 1 && (rc = smcb_uniform(c, us, n - 1))) return rc;
             u_in = us;
         }
-        k_ssp_counts<<<1, 32, 0, c->stream>>>(W, n, m, u_in, nr, status);
-        c->launches++;
-        SMCB_CUDA(cudaGetLastError());
+        SMCB_TRY(launch(c, k_ssp_counts, 1, 32, 0, W, n, m, u_in, nr, status));
         long long total = 0;
         SMCB_CUDA(cudaMemcpyAsync(&total, status, sizeof(total), cudaMemcpyDeviceToHost, c->stream));
         SMCB_CUDA(cudaStreamSynchronize(c->stream));
@@ -788,8 +758,7 @@ extern "C" int smcb_resample(smcb_ctx *c, int scheme, const double *W, int64_t n
             return SMCB_EINVAL;
         }
         if ((rc = run_scan<long long>(c, LoadCounts{nr}, n, cum))) return rc;
-        LAUNCH(c, k_repeat, grid_for(m, kBlock * 4), kBlock, cum, n, m, A_out);
-        return SMCB_OK;
+        return launch(c, k_repeat, grid_for(m, kBlock * 4), kBlock, 0, cum, n, m, A_out);
     }
     const int64_t nu = (scheme == SMCB_RS_SYSTEMATIC) ? 1 : (scheme == SMCB_RS_STRATIFIED ? m : m + 1);
     if (u_in == nullptr) {
@@ -807,14 +776,13 @@ extern "C" int smcb_resample(smcb_ctx *c, int scheme, const double *W, int64_t n
     if (scheme == SMCB_RS_RESIDUAL) {
         long long *cum_ip = reinterpret_cast<long long *>(aux);
         if ((rc = run_scan<long long>(c, LoadIntPart{W, (double)m}, n, cum_ip))) return rc;
-        LAUNCH(c, k_repeat, grid_for(m, kBlock * 4), kBlock, cum_ip, n, m, A_out);
+        SMCB_TRY(launch(c, k_repeat, grid_for(m, kBlock * 4), kBlock, 0, cum_ip, n, m, A_out));
         // residual weights res/sres -> cdf; spacings over (sres + 1) uniforms: only the first
         // sres + 1 entries of z are meaningful, and z[k]/z[sres] needs exactly those.
         if ((rc = run_scan<double>(c, LoadResidual{W, (double)m, cum_ip, n}, n, cdf))) return rc;
         if ((rc = run_scan<double>(c, LoadNegLog{u_in}, m + 1, z, 1))) return rc;
-        LAUNCH(c, k_search_residual, grid_for(m, kBlock * 4), kBlock, cdf, n,
-               SuSpacingsDyn{z, cum_ip, n, m}, A_out);
-        return SMCB_OK;
+        return launch(c, k_search_residual, grid_for(m, kBlock * 4), kBlock, 0, cdf, n, SuSpacingsDyn{z, cum_ip, n, m},
+                      A_out);
     }
     set_error("smcb_resample: %d is not a valid resampling scheme", scheme);
     return SMCB_EINVAL;
@@ -835,8 +803,7 @@ extern "C" int smcb_gather(smcb_ctx *c, const double *X, int64_t n, const int64_
                            int d, double *Xp) {
     SMCB_REQUIRE(c && X && A && Xp, "smcb_gather: NULL argument");
     SMCB_REQUIRE(n >= 1 && m >= 1 && d >= 1, "smcb_gather: bad sizes");
-    LAUNCH(c, k_gather, grid_for(m, kBlock * 4), kBlock, X, n, A, m, d, Xp);
-    return SMCB_OK;
+    return launch(c, k_gather, grid_for(m, kBlock * 4), kBlock, 0, X, n, A, m, d, Xp);
 }
 
 __global__ void __launch_bounds__(kBlock) k_gather_rows(const double *__restrict__ X, int64_t n,
@@ -855,8 +822,7 @@ extern "C" int smcb_gather_rows(smcb_ctx *c, const double *X, int64_t n, const i
                                 int64_t m, int d, double *Xp) {
     SMCB_REQUIRE(c && X && A && Xp, "smcb_gather_rows: NULL argument");
     SMCB_REQUIRE(n >= 1 && m >= 1 && d >= 1, "smcb_gather_rows: bad sizes");
-    LAUNCH(c, k_gather_rows, grid_for(m * d, kBlock * 4), kBlock, X, n, A, m, d, Xp);
-    return SMCB_OK;
+    return launch(c, k_gather_rows, grid_for(m * d, kBlock * 4), kBlock, 0, X, n, A, m, d, Xp);
 }
 
 // ---------------------------------------------------------------------------
@@ -904,17 +870,15 @@ extern "C" int smcb_normal_rvs(smcb_ctx *c, const double *loc, double loc0, cons
                                double scale0, const double *z_in, double *out, int64_t n) {
     SMCB_REQUIRE(c && out && n >= 1, "smcb_normal_rvs: bad argument");
     uint64_t call = z_in ? 0 : c->api_counter++;
-    LAUNCH(c, k_normal_rvs, grid_for((n + 1) / 2, kBlock * 4), kBlock, key_of(c->seed), call, loc, loc0,
-           scale, scale0, z_in, out, n);
-    return SMCB_OK;
+    return launch(c, k_normal_rvs, grid_for((n + 1) / 2, kBlock * 4), kBlock, 0, key_of(c->seed), call, loc, loc0,
+                  scale, scale0, z_in, out, n);
 }
 
 extern "C" int smcb_normal_logpdf(smcb_ctx *c, const double *x, double x0, const double *loc,
                                   double loc0, const double *scale, double scale0, double *out,
                                   int64_t n) {
     SMCB_REQUIRE(c && out && n >= 1, "smcb_normal_logpdf: bad argument");
-    LAUNCH(c, k_normal_logpdf, grid_for(n, kBlock * 4), kBlock, x, x0, loc, loc0, scale, scale0, out, n);
-    return SMCB_OK;
+    return launch(c, k_normal_logpdf, grid_for(n, kBlock * 4), kBlock, 0, x, x0, loc, loc0, scale, scale0, out, n);
 }
 
 // ---------------------------------------------------------------------------
@@ -955,8 +919,7 @@ __global__ void __launch_bounds__(kBlock) k_logpdf1(int kind, const double *__re
 extern "C" int smcb_logpdf1(smcb_ctx *c, int kind, const double *x, double x0, double p0, double c0, const double *p1,
                             double p10, const double *p2, double p20, double *out, int64_t n) {
     SMCB_REQUIRE(c && out && n >= 1 && kind >= 0 && kind <= 3, "smcb_logpdf1: bad argument");
-    LAUNCH(c, k_logpdf1, grid_for(n, kBlock * 4), kBlock, kind, x, x0, p0, c0, p1, p10, p2, p20, out, n);
-    return SMCB_OK;
+    return launch(c, k_logpdf1, grid_for(n, kBlock * 4), kBlock, 0, kind, x, x0, p0, c0, p1, p10, p2, p20, out, n);
 }
 
 constexpr int kMaxDim = 8;
@@ -1157,16 +1120,14 @@ extern "C" int smcb_mvnormal_rvs(smcb_ctx *c, const double *loc, const double *l
         MvnBig B;
         int rc = fill_mvn_big(c, &B, loc0, scale0, L, d);
         if (rc) return rc;
-        LAUNCH(c, k_mvn_big<false>, grid_for(n, kBlock), kBlock, key_of(c->seed), call, B, (const double *)nullptr, loc,
-               scale, z_in, out, n);
-        return SMCB_OK;
+        return launch(c, k_mvn_big<false>, grid_for(n, kBlock), kBlock, 0, key_of(c->seed), call, B,
+                      (const double *)nullptr, loc, scale, z_in, out, n);
     }
     MvnParams P;
     int rc = fill_mvn(&P, loc0, scale0, L, d);
     if (rc) return rc;
-    LAUNCH(c, k_mvn_rvs, grid_for((n + 1) / 2, kBlock * 2), kBlock, key_of(c->seed), call, P, loc, scale,
-           z_in, out, n);
-    return SMCB_OK;
+    return launch(c, k_mvn_rvs, grid_for((n + 1) / 2, kBlock * 2), kBlock, 0, key_of(c->seed), call, P, loc, scale,
+                  z_in, out, n);
 }
 
 extern "C" int smcb_mvnormal_logpdf(smcb_ctx *c, const double *x, const double *loc,
@@ -1177,15 +1138,13 @@ extern "C" int smcb_mvnormal_logpdf(smcb_ctx *c, const double *x, const double *
         MvnBig B;
         int rc = fill_mvn_big(c, &B, loc0, scale0, L, d);
         if (rc) return rc;
-        LAUNCH(c, k_mvn_big<true>, grid_for(n, kBlock), kBlock, key_of(c->seed), 0ull, B, x, loc, scale,
-               (const double *)nullptr, out, n);
-        return SMCB_OK;
+        return launch(c, k_mvn_big<true>, grid_for(n, kBlock), kBlock, 0, key_of(c->seed), 0ull, B, x, loc, scale,
+                      (const double *)nullptr, out, n);
     }
     MvnParams P;
     int rc = fill_mvn(&P, loc0, scale0, L, d);
     if (rc) return rc;
-    LAUNCH(c, k_mvn_logpdf, grid_for(n, kBlock * 2), kBlock, P, x, loc, scale, out, n);
-    return SMCB_OK;
+    return launch(c, k_mvn_logpdf, grid_for(n, kBlock * 2), kBlock, 0, P, x, loc, scale, out, n);
 }
 
 // ---------------------------------------------------------------------------
@@ -1220,11 +1179,9 @@ extern "C" int smcb_device_math(smcb_ctx *c, int fn, const double *x, double *ou
     SMCB_REQUIRE(c && x && out && n >= 1 && fn >= 0 && fn <= 8, "smcb_device_math: bad argument");
     static bool attr_set = false;
     if (!attr_set) {
-        SMCB_CUDA(cudaFuncSetAttribute(k_device_math, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMathTabBytes));
+        SMCB_TRY(set_smem(k_device_math, kMathTabBytes));
         attr_set = true;
     }
-    k_device_math<<<grid_for(n, kBlock * 4), kBlock, fn >= 4 ? kMathTabBytes : 0, c->stream>>>(fn, x, out, n, c->math_tab);
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    return launch(c, k_device_math, grid_for(n, kBlock * 4), kBlock, fn >= 4 ? kMathTabBytes : 0, fn, x, out, n,
+                  c->math_tab);
 }

@@ -268,7 +268,7 @@ __global__ void k_bank_keys(uint64_t *key, int64_t n, uint64_t seed, uint64_t co
 template <class M, int FK, int SCHEME, bool RES>
 static int bank_kernel_setup(smcb_ctx *c, int64_t nrun, size_t smem, int &grid) {
     auto kern = k_bank<M, FK, SCHEME, RES>;
-    SMCB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SMCB_TRY(set_smem(kern, smem));
     int nb = 0, sms = 0;
     SMCB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kBatchBS, smem));
     SMCB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
@@ -312,12 +312,8 @@ static int bank_one(smcb_ctx *c, const smcb_bank_desc &d, int64_t *out) {
                  "smcb_bank_advance: the streaming tier needs %d scratch rows (got %lld)", grid,
                  (long long)d.scratch_rows);
     if (tier == SMCB_BATCH_RESIDENT)
-        k_bank<M, FK, SCHEME, true><<<grid, kBatchBS, smem_res, c->stream>>>(d, c->math_tab);
-    else
-        k_bank<M, FK, SCHEME, false><<<grid, kBatchBS, kMathTabBytes, c->stream>>>(d, c->math_tab);
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+        return launch(c, k_bank<M, FK, SCHEME, true>, grid, kBatchBS, smem_res, d, c->math_tab);
+    return launch(c, k_bank<M, FK, SCHEME, false>, grid, kBatchBS, kMathTabBytes, d, c->math_tab);
 }
 
 static int bank_dispatch(smcb_ctx *c, const smcb_bank_desc *dp, int64_t *out) {
@@ -387,12 +383,9 @@ extern "C" int smcb_bank_gather(smcb_ctx *c, const smcb_bank_desc *src, const in
                  (long long)dst->R, (long long)m);
     if (m == 0 || src->R == 0) return SMCB_OK;
     auto *f = reinterpret_cast<unsigned long long *>(first);
-    k_first_fill<<<grid_for(src->R, 256), 256, 0, c->stream>>>(f, src->R);
-    k_first_min<<<grid_for(m, 256), 256, 0, c->stream>>>(A, m, f);
-    k_bank_rows<<<rows_grid(m), kRowBS, 0, c->stream>>>(*src, *dst, A, nullptr, f, seed, counter, m);
-    c->launches += 3;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    SMCB_TRY(launch(c, k_first_fill, grid_for(src->R, 256), 256, 0, f, src->R));
+    SMCB_TRY(launch(c, k_first_min, grid_for(m, 256), 256, 0, A, m, f));
+    return launch(c, k_bank_rows, rows_grid(m), kRowBS, 0, *src, *dst, A, nullptr, f, seed, counter, m);
 }
 
 extern "C" int smcb_bank_merge(smcb_ctx *c, const smcb_bank_desc *dst, const smcb_bank_desc *src,
@@ -403,17 +396,11 @@ extern "C" int smcb_bank_merge(smcb_ctx *c, const smcb_bank_desc *dst, const smc
     SMCB_REQUIRE(src->R == dst->R, "smcb_bank_merge: %lld proposals for %lld slots", (long long)src->R,
                  (long long)dst->R);
     if (dst->R == 0) return SMCB_OK;
-    k_bank_rows<<<rows_grid(dst->R), kRowBS, 0, c->stream>>>(*src, *dst, nullptr, accepted, nullptr, 0, 0, dst->R);
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    return launch(c, k_bank_rows, rows_grid(dst->R), kRowBS, 0, *src, *dst, nullptr, accepted, nullptr, 0, 0, dst->R);
 }
 
 extern "C" int smcb_bank_keys(smcb_ctx *c, uint64_t *key, int64_t n, uint64_t seed, uint64_t counter) {
     SMCB_REQUIRE(c && key && n >= 0, "smcb_bank_keys: bad argument");
     if (n == 0) return SMCB_OK;
-    k_bank_keys<<<grid_for(n, 256), 256, 0, c->stream>>>(key, n, seed, counter);
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    return launch(c, k_bank_keys, grid_for(n, 256), 256, 0, key, n, seed, counter);
 }

@@ -216,7 +216,7 @@ __global__ void __launch_bounds__(kBatchBS) k_batch(const smcb_batch_desc d, con
 template <class M, int FK, int SCHEME, bool RES>
 static int batch_kernel_setup(smcb_ctx *c, const smcb_batch_desc &d, size_t smem, int &grid) {
     auto kern = k_batch<M, FK, SCHEME, RES>;
-    SMCB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SMCB_TRY(set_smem(kern, smem));
     int nb = 0, sms = 0;
     SMCB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kBatchBS, smem));
     SMCB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
@@ -255,12 +255,8 @@ static int batch_one(smcb_ctx *c, const smcb_batch_desc &d, int64_t *out) {
     SMCB_REQUIRE(tier == SMCB_BATCH_RESIDENT || (d.cdf && (SCHEME != SMCB_RS_MULTINOMIAL || d.scratch)),
                  "smcb_batch_run: the streaming tier needs cdf (and scratch for multinomial)");
     if (tier == SMCB_BATCH_RESIDENT)
-        k_batch<M, FK, SCHEME, true><<<grid, kBatchBS, smem_res, c->stream>>>(d, c->math_tab);
-    else
-        k_batch<M, FK, SCHEME, false><<<grid, kBatchBS, kMathTabBytes, c->stream>>>(d, c->math_tab);
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+        return launch(c, k_batch<M, FK, SCHEME, true>, grid, kBatchBS, smem_res, d, c->math_tab);
+    return launch(c, k_batch<M, FK, SCHEME, false>, grid, kBatchBS, kMathTabBytes, d, c->math_tab);
 }
 
 template <class M, int FK>

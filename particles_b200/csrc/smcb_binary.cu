@@ -20,15 +20,9 @@
 // CTA.  A pivot that is not positive (where scipy.linalg.cholesky raises LinAlgError) gives llik = -inf and sets
 // bit 0 of *err; it never yields a NaN silently.  All arithmetic is fp64.
 #include "smcb_common.cuh"
+#include "smcb_reduce.cuh"
 
 using namespace smcb;
-
-#define LAUNCHB(ctx, kern, grid, block, smem, ...)                               \
-    do {                                                                         \
-        kern<<<(grid), (block), (smem), (ctx)->stream>>>(__VA_ARGS__);           \
-        (ctx)->launches++;                                                       \
-        SMCB_CUDA(cudaGetLastError());                                           \
-    } while (0)
 
 namespace smcb {
 
@@ -36,19 +30,11 @@ constexpr int kBinMaxP = 128;
 constexpr int kBinWords = kBinMaxP / 32;
 constexpr int kBinThreads = 128;                   // smcb_nested_logistic
 constexpr size_t kBinSmemBudget = 200 * 1024;      // of the 227 KB a CTA may use
-// Philox purposes (counter word 3, low byte), distinct from smcb_common.cuh's
-constexpr uint32_t kPurposeBinProp = 4, kPurposeBinAcc = 5, kPurposeBinRvs = 6;
 
 __host__ __device__ __forceinline__ int tri(int a) { return a * (a + 1) / 2; }
 
 __device__ __forceinline__ double log_no_warn(double x) { return log(x > 1e-300 ? x : 1e-300); }   // :62-64
 __device__ __forceinline__ double expit(double x) { return 1.0 / (1.0 + exp(-x)); }
-
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-    for (int m = 16; m > 0; m >>= 1) v += __shfl_xor_sync(0xffffffffu, v, m);
-    return v;
-}
 
 // the uniform of coordinate i of particle / chain n at step s (s = 0: smcb_nested_logistic)
 __device__ __forceinline__ double bin_uniform(const Philox &key, uint64_t n, uint64_t call, int s, int i,
@@ -354,12 +340,11 @@ extern "C" int smcb_vs_loglik(smcb_ctx *c, const smcb_vs_desc *m, const uint8_t 
     SMCB_REQUIRE(!lpost || (lprior && llik), "smcb_vs_loglik: lpost needs lprior and llik");
     const int wpc = bin_warps(kmax);
     const size_t smem = bin_smem(kmax, wpc);
-    SMCB_CUDA(cudaFuncSetAttribute(k_vs_loglik, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SMCB_TRY(set_smem(k_vs_loglik, smem));
     const int64_t grid = (n + wpc - 1) / wpc;
     SMCB_REQUIRE(grid < (1ll << 31), "smcb_vs_loglik: too many particles");
-    LAUNCHB(c, k_vs_loglik, (unsigned)grid, 32 * wpc, smem, *m, gamma, n, kmax, vm2, epn, len_gam, ldet, wtw, lprior,
-            llik, lpost, err);
-    return SMCB_OK;
+    return launch(c, k_vs_loglik, (unsigned)grid, 32 * wpc, smem, *m, gamma, n, kmax, vm2, epn, len_gam, ldet, wtw,
+                  lprior, llik, lpost, err);
 }
 
 extern "C" int smcb_nested_logistic(smcb_ctx *c, int p, const double *coeffs, const uint8_t *edgy, int64_t n,
@@ -369,13 +354,8 @@ extern "C" int smcb_nested_logistic(smcb_ctx *c, int p, const double *coeffs, co
     SMCB_REQUIRE(draw || logpdf, "smcb_nested_logistic: nothing to compute");
     const int64_t grid = (n + kBinThreads - 1) / kBinThreads;
     const uint64_t call = (draw && !u_in) ? c->api_counter++ : 0;
-    if (draw)
-        LAUNCHB(c, k_nested_logistic<true>, (unsigned)grid, kBinThreads, 0, p, coeffs, edgy, n, x, u_in,
-                key_of(c->seed), call, logpdf);
-    else
-        LAUNCHB(c, k_nested_logistic<false>, (unsigned)grid, kBinThreads, 0, p, coeffs, edgy, n, x, u_in,
-                key_of(c->seed), call, logpdf);
-    return SMCB_OK;
+    return launch(c, draw ? k_nested_logistic<true> : k_nested_logistic<false>, (unsigned)grid, kBinThreads, 0, p,
+                  coeffs, edgy, n, x, u_in, key_of(c->seed), call, logpdf);
 }
 
 extern "C" int smcb_binary_wf_move(smcb_ctx *c, const smcb_vs_desc *m, const double *coeffs, const uint8_t *edgy,
@@ -390,10 +370,10 @@ extern "C" int smcb_binary_wf_move(smcb_ctx *c, const smcb_vs_desc *m, const dou
     SMCB_REQUIRE((u_prop == nullptr) == (u_acc == nullptr), "smcb_binary_wf_move: inject both uniforms or neither");
     const int wpc = bin_warps(m->p);
     const size_t smem = bin_smem(m->p, wpc);
-    SMCB_CUDA(cudaFuncSetAttribute(k_binary_wf_move, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SMCB_TRY(set_smem(k_binary_wf_move, smem));
     const int64_t grid = (M + wpc - 1) / wpc;
     const uint64_t call = u_prop ? 0 : c->api_counter++;
-    LAUNCHB(c, k_binary_wf_move, (unsigned)grid, 32 * wpc, smem, *m, coeffs, edgy, M, P, epn, x0, lprior0, llik0,
-            lpost0, key_of(c->seed), call, u_prop, u_acc, x_out, lprior_out, llik_out, lpost_out, pb_out, err);
-    return SMCB_OK;
+    return launch(c, k_binary_wf_move, (unsigned)grid, 32 * wpc, smem, *m, coeffs, edgy, M, P, epn, x0, lprior0,
+                  llik0, lpost0, key_of(c->seed), call, u_prop, u_acc, x_out, lprior_out, llik_out, lpost_out, pb_out,
+                  err);
 }

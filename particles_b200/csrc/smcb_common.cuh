@@ -35,6 +35,14 @@ void set_error(const char *fmt, ...);
             return SMCB_EINVAL;                                                  \
         }                                                                        \
     } while (0)
+// returns from the caller with expr's code unless it is SMCB_OK
+#define SMCB_TRY(expr)                                                           \
+    do {                                                                         \
+        const int smcb_rc_ = (expr);                                             \
+        if (smcb_rc_ != SMCB_OK) return smcb_rc_;                                \
+    } while (0)
+
+constexpr unsigned kFull = 0xffffffffu;   // every lane of a warp
 
 inline int grid_for(int64_t work_items, int items_per_block) {
     int64_t b = (work_items + items_per_block - 1) / items_per_block;
@@ -86,8 +94,22 @@ __device__ __forceinline__ void philox4x32_10k(uint32_t c0, uint32_t c1, uint32_
     out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
 }
 
-// purposes (counter word 3, low byte) so that streams never collide
-enum : uint32_t { kPurposeNormal = 1, kPurposeUniform = 2, kPurposeApi = 3 };
+// Philox purposes: the low byte of counter word 3, so that streams never collide.  Pick a new feature's value here.
+// The values used twice are kept apart by another counter word or by the key:
+//   4, 5  the backward samplers (Smooth*) and the binary-space kernels (Bin*) both key on the context seed and put the
+//         API call number, which every random entry point takes afresh from smcb_ctx::api_counter, in word 2;
+//         the on-line smoothers' 5 is under their own key, seed ^ kOnlineSeedMix.
+//   6     the binary-space draws (BinRvs) key on the context seed, the conditional SMC trajectory (Traj) on the
+//         filter bank's per-filter keys.
+enum : uint32_t {
+    kPurposeNormal = 1, kPurposeUniform = 2, kPurposeApi = 3,
+    kPurposeSmooth = 4,       // a backward draw's proposal + acceptance uniforms of trial `trial`
+    kPurposeSmoothExact = 5,  // the uniform of an exact O(N) backward draw
+    kPurposeBinProp = 4, kPurposeBinAcc = 5, kPurposeBinRvs = 6,
+    kPurposeTraj = 6,         // the uniform of the conditional SMC trajectory draw at step t
+    kPurposeHmm = 7,          // the uniform of trajectory n's draw at step t of HMM b
+};
+constexpr uint64_t kOnlineSeedMix = 0x9E3779B97F4A7C15ull;   // the on-line smoothers' key: seed ^ kOnlineSeedMix
 
 // 53-bit uniform in [0, 1), the construction numpy's legacy rand uses
 __host__ __device__ __forceinline__ double u53(uint32_t a, uint32_t b) {
@@ -268,5 +290,26 @@ __host__ __device__ inline Philox key_of(uint64_t seed) {
         k.rk[2 * r + 1] = k.k1 + (uint32_t)r * 0xBB67AE85u;
     }
     return k;
+}
+
+// Launches kern on the context's stream and counts it in ctx->launches (smcb_launch_count).  A launch the runtime
+// rejects returns SMCB_ECUDA at once, so no later launch of the same entry point runs on its missing results.
+template <class... P, class... A>
+int launch(smcb_ctx *ctx, void (*kern)(P...), dim3 grid, dim3 block, size_t smem, A &&...args) {
+    kern<<<grid, block, smem, ctx->stream>>>(static_cast<A &&>(args)...);
+    ctx->launches++;
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) {
+        set_error("kernel launch: %s", cudaGetErrorString(e));
+        return SMCB_ECUDA;
+    }
+    return SMCB_OK;
+}
+
+// lets launches of `kern` use `bytes` of dynamic shared memory
+template <class K>
+int set_smem(K kern, size_t bytes) {
+    SMCB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    return SMCB_OK;
 }
 }  // namespace smcb

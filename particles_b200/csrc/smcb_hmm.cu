@@ -14,13 +14,13 @@
 // fexp_neg, log the CUDA fp64 log, and the library is compiled with -fmad=false.
 // Randomness (SAMPLE without injected uniforms): Philox keyed by the descriptor's seed, counter (n, t, b,
 // kPurposeHmm): the draws do not depend on the tile size or the launch shape.
-#include "smcb_smooth.cuh"
+#include "smcb_math.cuh"
+#include "smcb_reduce.cuh"
 
 using namespace smcb;
 
 namespace {
 
-constexpr uint32_t kPurposeHmm = 7;            // the uniform of trajectory n's draw at step t of HMM b
 constexpr int kHmmGroups = 4;                  // warp tier: HMMs (one warp each) per CTA
 constexpr int kSampleBlock = 256;              // SAMPLE: trajectories per CTA
 
@@ -43,16 +43,8 @@ struct Group {
         __syncthreads();
         return r;
     }
-    __device__ __forceinline__ double sum(double v) const {
-#pragma unroll
-        for (int mask = 16; mask > 0; mask >>= 1) v += __shfl_xor_sync(kFull, v, mask);
-        return across_warps(v, false);
-    }
-    __device__ __forceinline__ double max(double v) const {
-#pragma unroll
-        for (int mask = 16; mask > 0; mask >>= 1) v = fmax(v, __shfl_xor_sync(kFull, v, mask));
-        return across_warps(v, true);
-    }
+    __device__ __forceinline__ double sum(double v) const { return across_warps(warp_sum(v), false); }
+    __device__ __forceinline__ double max(double v) const { return across_warps(warp_max(v), true); }
 };
 
 // the group of this thread: which HMM, which state, where its shared-memory slab (`per` doubles) starts
@@ -223,15 +215,12 @@ int launch_groups(smcb_ctx *c, const smcb_hmm_desc &d) {
     const int block = kWarp ? 32 * kHmmGroups : 32 * ((K + 31) / 32);
     const size_t smem = kWarp ? per * kHmmGroups : per;
     const int64_t grid = kWarp ? (d.B + kHmmGroups - 1) / kHmmGroups : d.B;
-    int rc;
     if (d.method == SMCB_HMM_FORWARD) {
-        if ((rc = set_smem(k_hmm_forward<kWarp>, smem)) != SMCB_OK) return rc;
-        k_hmm_forward<kWarp><<<(unsigned)grid, block, smem, c->stream>>>(d);
-    } else {
-        if ((rc = set_smem(k_hmm_backward<kWarp>, smem)) != SMCB_OK) return rc;
-        k_hmm_backward<kWarp><<<(unsigned)grid, block, smem, c->stream>>>(d);
+        SMCB_TRY(set_smem(k_hmm_forward<kWarp>, smem));
+        return launch(c, k_hmm_forward<kWarp>, (unsigned)grid, block, smem, d);
     }
-    return SMCB_OK;
+    SMCB_TRY(set_smem(k_hmm_backward<kWarp>, smem));
+    return launch(c, k_hmm_backward<kWarp>, (unsigned)grid, block, smem, d);
 }
 
 }  // namespace
@@ -248,27 +237,22 @@ extern "C" int smcb_hmm(smcb_ctx *c, const smcb_hmm_desc *dp) {
     SMCB_REQUIRE(d.K >= 1 && d.B >= 1 && d.B <= 0x7fffffffLL && d.ld >= 1, "smcb_hmm: bad sizes K=%d B=%lld ld=%lld",
                  (int)d.K, (long long)d.B, (long long)d.ld);
     SMCB_REQUIRE(d.trans && d.trans_stride >= 0 && d.filt && d.logft, "smcb_hmm: NULL trans, filt or logft");
-    int rc = SMCB_OK;
     if (d.method == SMCB_HMM_FORWARD) {
         SMCB_REQUIRE(d.init && d.init_stride >= 0 && d.pred && d.logpyt, "smcb_hmm: FORWARD needs init, pred, logpyt");
         SMCB_REQUIRE(d.t0 >= 0 && d.t0 <= d.t1 && d.t1 <= d.ld, "smcb_hmm: bad rows [%lld, %lld) of %lld",
                      (long long)d.t0, (long long)d.t1, (long long)d.ld);
         if (d.t0 == d.t1) return SMCB_OK;
-        rc = d.K <= 32 ? launch_groups<true>(c, d) : launch_groups<false>(c, d);
-    } else if (d.method == SMCB_HMM_BACKWARD) {
-        SMCB_REQUIRE(d.smth && d.t1 >= 1 && d.t1 <= d.ld, "smcb_hmm: BACKWARD needs smth and 1 <= T <= ld");
-        rc = d.K <= 32 ? launch_groups<true>(c, d) : launch_groups<false>(c, d);
-    } else {
-        SMCB_REQUIRE(d.paths && d.t1 >= 1 && d.t1 <= d.ld && d.N >= 1 && d.N <= 0x7fffffffLL && d.B <= 65535,
-                     "smcb_hmm: SAMPLE needs paths, 1 <= T <= ld, 1 <= N < 2^31 and B <= 65535");
-        if (d.t1 == 1) return SMCB_OK;
-        const size_t smem = ((size_t)d.K * d.K + d.K) * sizeof(double);
-        if ((rc = set_smem(k_hmm_sample, smem)) != SMCB_OK) return rc;
-        const dim3 grid((unsigned)((d.N + kSampleBlock - 1) / kSampleBlock), (unsigned)d.B);
-        k_hmm_sample<<<grid, kSampleBlock, smem, c->stream>>>(d, key_of(d.seed));
+        return d.K <= 32 ? launch_groups<true>(c, d) : launch_groups<false>(c, d);
     }
-    if (rc != SMCB_OK) return rc;
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    if (d.method == SMCB_HMM_BACKWARD) {
+        SMCB_REQUIRE(d.smth && d.t1 >= 1 && d.t1 <= d.ld, "smcb_hmm: BACKWARD needs smth and 1 <= T <= ld");
+        return d.K <= 32 ? launch_groups<true>(c, d) : launch_groups<false>(c, d);
+    }
+    SMCB_REQUIRE(d.paths && d.t1 >= 1 && d.t1 <= d.ld && d.N >= 1 && d.N <= 0x7fffffffLL && d.B <= 65535,
+                 "smcb_hmm: SAMPLE needs paths, 1 <= T <= ld, 1 <= N < 2^31 and B <= 65535");
+    if (d.t1 == 1) return SMCB_OK;
+    const size_t smem = ((size_t)d.K * d.K + d.K) * sizeof(double);
+    SMCB_TRY(set_smem(k_hmm_sample, smem));
+    const dim3 grid((unsigned)((d.N + kSampleBlock - 1) / kSampleBlock), (unsigned)d.B);
+    return launch(c, k_hmm_sample, grid, kSampleBlock, smem, d, key_of(d.seed));
 }

@@ -11,7 +11,7 @@
 // index order inside one thread, from 0.0, and nothing depends on where the model sits in the batch, so a batch row
 // is bit-identical to the same model run alone; the library is compiled with -fmad=false.  A non-positive pivot in a
 // Cholesky factor becomes NaN, which then fills that model's rows from that step on (no host read, no exception).
-#include "smcb_smooth.cuh"
+#include "smcb_common.cuh"
 
 using namespace smcb;
 
@@ -352,22 +352,12 @@ extern "C" int smcb_kalman(smcb_ctx *c, const smcb_kalman_desc *dp) {
     const bool filter = d.method == SMCB_KALMAN_FILTER;
     if (d.dx == 1 && d.dy == 1) {
         const unsigned grid = (unsigned)((d.B + kScalarBlock - 1) / kScalarBlock);
-        if (filter) k_kalman_filter_1<<<grid, kScalarBlock, 0, c->stream>>>(d);
-        else k_kalman_smooth_1<<<grid, kScalarBlock, 0, c->stream>>>(d);
-    } else {
-        const int g = warp_groups(d.dx, d.dy);
-        const size_t smem = (size_t)g * slab_doubles(d.dx, d.dy) * sizeof(double);
-        const unsigned grid = (unsigned)((d.B + g - 1) / g);
-        int rc;
-        if (filter) {
-            if ((rc = set_smem(k_kalman_filter_w, smem)) != SMCB_OK) return rc;
-            k_kalman_filter_w<<<grid, 32 * g, smem, c->stream>>>(d);
-        } else {
-            if ((rc = set_smem(k_kalman_smooth_w, smem)) != SMCB_OK) return rc;
-            k_kalman_smooth_w<<<grid, 32 * g, smem, c->stream>>>(d);
-        }
+        return launch(c, filter ? k_kalman_filter_1 : k_kalman_smooth_1, grid, kScalarBlock, 0, d);
     }
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    const int g = warp_groups(d.dx, d.dy);
+    const size_t smem = (size_t)g * slab_doubles(d.dx, d.dy) * sizeof(double);
+    const unsigned grid = (unsigned)((d.B + g - 1) / g);
+    const auto kern = filter ? k_kalman_filter_w : k_kalman_smooth_w;
+    SMCB_TRY(set_smem(kern, smem));
+    return launch(c, kern, grid, 32 * g, smem, d);
 }

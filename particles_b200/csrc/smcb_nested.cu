@@ -15,6 +15,7 @@
 // Every reduction is deterministic: integer counts and integer min / max are order-free, and the floating-point
 // sums run grid-stride over a grid that depends on n only, then over the warps and the blocks in a fixed order.
 #include "smcb_common.cuh"
+#include "smcb_reduce.cuh"
 
 using namespace smcb;
 
@@ -50,17 +51,6 @@ __device__ __forceinline__ double ns_value(unsigned long long k) {
     return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
 }
 
-// "last block" ticket of a grid-stride pass: true in the block that finishes last
-__device__ __forceinline__ bool ns_last_block(unsigned int *ticket) {
-    __shared__ bool last;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) last = atomicInc(ticket, gridDim.x - 1) == gridDim.x - 1;
-    __syncthreads();
-    if (last) __threadfence();
-    return last;
-}
-
 // one radix-select pass: the histogram of the digit at `shift` over the keys whose bits above the digit equal the
 // prefix's; the last block finds the bucket of rank st->rank, extends the prefix and clears the histogram.
 // prefix and rank are read once, at the start: every block reads them before the last block (the one that has seen
@@ -90,7 +80,7 @@ __global__ void __launch_bounds__(kNsBlock) k_ns_select_pass(const double *__res
     __syncthreads();
     for (int b = threadIdx.x; b < kNsBins; b += kNsBlock)
         if (s_hist[b]) atomicAdd(&hist[b], s_hist[b]);
-    if (!ns_last_block(ticket)) return;
+    if (!last_block(ticket)) return;
     // each thread owns kNsBinsPerThread consecutive bins; a serial scan over the threads' sums finds the owner
     unsigned long long own = 0ull;
     unsigned int cnt[kNsBinsPerThread];
@@ -124,16 +114,6 @@ __global__ void __launch_bounds__(kNsBlock) k_ns_select_pass(const double *__res
     for (int j = 0; j < kNsBinsPerThread; j++) hist[threadIdx.x * kNsBinsPerThread + j] = 0u;
 }
 
-__device__ __forceinline__ unsigned long long warp_min_u64(unsigned long long v) {
-    for (int m = 16; m > 0; m >>= 1) { const unsigned long long o = __shfl_xor_sync(0xffffffffu, v, m); v = o < v ? o : v; }
-    return v;
-}
-
-__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
-    for (int m = 16; m > 0; m >>= 1) { const unsigned long long o = __shfl_xor_sync(0xffffffffu, v, m); v = o > v ? o : v; }
-    return v;
-}
-
 // the smallest key above statistic k0 and the largest key; the last block forms lt (numpy's _lerp, nested.py:332)
 __global__ void __launch_bounds__(kNsBlock) k_ns_level(const double *__restrict__ llik, int64_t n, int64_t k1,
                                                       double gamma, NsState *st, unsigned int *ticket) {
@@ -144,13 +124,13 @@ __global__ void __launch_bounds__(kNsBlock) k_ns_level(const double *__restrict_
         if (k > a_key && k < nx) nx = k;
         if (k > mx) mx = k;
     }
-    nx = warp_min_u64(nx);
-    mx = warp_max_u64(mx);
+    nx = warp_min(nx);
+    mx = warp_max(mx);
     if ((threadIdx.x & 31) == 0) {
         if (nx != ~0ull) atomicMin(&st->next_key, nx);
         atomicMax(&st->max_key, mx);
     }
-    if (!ns_last_block(ticket) || threadIdx.x != 0) return;
+    if (!last_block(ticket) || threadIdx.x != 0) return;
     const double a = ns_value(a_key);
     const unsigned long long nk = reinterpret_cast<volatile NsState *>(st)->next_key;
     // statistic k1 is statistic k0 while k1 falls inside k0's block of ties
@@ -167,7 +147,7 @@ __global__ void __launch_bounds__(kNsBlock) k_ns_cut_max(const double *__restric
         const double v = llik[i];
         if (v <= lt) { const unsigned long long k = ns_key(v); mx = k > mx ? k : mx; }
     }
-    mx = warp_max_u64(mx);
+    mx = warp_max(mx);
     if ((threadIdx.x & 31) == 0 && mx) atomicMax(&st->cut_key, mx);
 }
 
@@ -194,10 +174,8 @@ __global__ void __launch_bounds__(kNsBlock) k_ns_evidence(const double *__restri
         sc += exp(((v <= lt) ? v : -CUDART_INF) - mc);
         sa += exp(v - ma);
     }
-    for (int m = 16; m > 0; m >>= 1) {
-        sc += __shfl_xor_sync(0xffffffffu, sc, m);
-        sa += __shfl_xor_sync(0xffffffffu, sa, m);
-    }
+    sc = warp_sum(sc);
+    sa = warp_sum(sa);
     if ((threadIdx.x & 31) == 0) { s_red[0][threadIdx.x >> 5] = sc; s_red[1][threadIdx.x >> 5] = sa; }
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -206,7 +184,7 @@ __global__ void __launch_bounds__(kNsBlock) k_ns_evidence(const double *__restri
         partials[2 * blockIdx.x] = c;
         partials[2 * blockIdx.x + 1] = a;
     }
-    if (!ns_last_block(ticket) || threadIdx.x != 0) return;
+    if (!last_block(ticket) || threadIdx.x != 0) return;
     double c = 0.0, a = 0.0;
     for (unsigned int b = 0; b < gridDim.x; b++) {
         c += reinterpret_cast<volatile double *>(partials)[2 * b];
@@ -231,13 +209,6 @@ __global__ void __launch_bounds__(kNsBlock) k_ns_weights(const double *__restric
 
 }  // namespace smcb
 
-#define LAUNCHN(ctx, kern, grid, ...)                                            \
-    do {                                                                         \
-        kern<<<(grid), kNsBlock, 0, (ctx)->stream>>>(__VA_ARGS__);               \
-        (ctx)->launches++;                                                       \
-        SMCB_CUDA(cudaGetLastError());                                           \
-    } while (0)
-
 // NestedSamplingSMC.logG (nested.py:330-351) on the device: see the top of this file and include/smcb.h
 extern "C" int smcb_ns_threshold(smcb_ctx *c, const double *llik, int64_t n, int64_t k0, int64_t k1, double gamma,
                                  int t, double log_alpha, double log_evid, double eps, double *lw, double *out) {
@@ -259,11 +230,12 @@ extern "C" int smcb_ns_threshold(smcb_ctx *c, const double *llik, int64_t n, int
         const int top = 64 - p * kNsDigit;                               // the digit is bits [shift, top)
         const int shift = top > kNsDigit ? top - kNsDigit : 0;
         const unsigned long long hi_mask = (top == 64) ? 0ull : (~0ull << top);
-        LAUNCHN(c, k_ns_select_pass, grid, llik, n, shift, hi_mask, st, hist, c->counters + 12);
+        SMCB_TRY(launch(c, k_ns_select_pass, grid, kNsBlock, 0, llik, n, shift, hi_mask, st, hist,
+                        c->counters + kTicketNsSelect));
     }
-    LAUNCHN(c, k_ns_level, grid, llik, n, k1, gamma, st, c->counters + 13);
-    LAUNCHN(c, k_ns_cut_max, grid, llik, n, st);
-    LAUNCHN(c, k_ns_evidence, grid, llik, n, t, log_alpha, log_evid, eps, st, partials, c->counters + 14, out);
-    LAUNCHN(c, k_ns_weights, grid, llik, n, st, lw);
-    return SMCB_OK;
+    SMCB_TRY(launch(c, k_ns_level, grid, kNsBlock, 0, llik, n, k1, gamma, st, c->counters + kTicketNsLevel));
+    SMCB_TRY(launch(c, k_ns_cut_max, grid, kNsBlock, 0, llik, n, st));
+    SMCB_TRY(launch(c, k_ns_evidence, grid, kNsBlock, 0, llik, n, t, log_alpha, log_evid, eps, st, partials,
+                    c->counters + kTicketNsEvidence, out));
+    return launch(c, k_ns_weights, grid, kNsBlock, 0, llik, n, st, lw);
 }

@@ -15,7 +15,6 @@ using namespace smcb;
 
 namespace {
 
-constexpr uint64_t kOnlineSeedMix = 0x9E3779B97F4A7C15ull;   // separates these streams from the filter's
 constexpr int kOnRows = 4;                                    // ON2_W: rows per CTA
 constexpr int kOnWarps = kSmBlock / 32;
 
@@ -129,7 +128,7 @@ __global__ void __launch_bounds__(kSmBlock) k_paris(M m, smcb_online_desc d, Phi
             }
         }
     }
-    const long long na = warp_sum((live && acc) ? 1 : 0), np = warp_sum(nprop);
+    const long long na = warp_sum((live && acc) ? 1LL : 0LL), np = warp_sum(nprop);
     if (lane == 0) {
         atomicAdd(reinterpret_cast<unsigned long long *>(d.counts), (unsigned long long)na);
         atomicAdd(reinterpret_cast<unsigned long long *>(d.counts + 1), (unsigned long long)np);
@@ -198,11 +197,7 @@ __global__ void __launch_bounds__(kSmBlock) k_on2_weights(M m, smcb_online_desc 
     }
 #pragma unroll
     for (int r = 0; r < kOnRows; r++) {
-#pragma unroll
-        for (int mask = 16; mask > 0; mask >>= 1) {
-            const double mo = __shfl_xor_sync(kFull, mx[r], mask), so = __shfl_xor_sync(kFull, s[r], mask);
-            lse_merge(mx[r], s[r], mo, so);
-        }
+        warp_lse_merge(mx[r], s[r]);
         if (lane == 0) {
             s_part[0][warp][r] = mx[r];
             s_part[1][warp][r] = s[r];
@@ -266,13 +261,11 @@ __global__ void __launch_bounds__(kBlock) k_phi_on2(smcb_online_desc d) {
     const double *w = d.omega + r * N;
     double sw = 0.0;
     for (int64_t i = lane; i < N; i += 32) sw += w[i];
-#pragma unroll
-    for (int mask = 16; mask > 0; mask >>= 1) sw += __shfl_xor_sync(kFull, sw, mask);
+    sw = warp_sum(sw);
     for (int64_t c = 0; c < K; c++) {
         double acc = 0.0;
         for (int64_t i = lane; i < N; i += 32) acc += w[i] * (d.phi_prev[i * K + c] + d.psi[(r * N + i) * K + c]);
-#pragma unroll
-        for (int mask = 16; mask > 0; mask >>= 1) acc += __shfl_xor_sync(kFull, acc, mask);
+        acc = warp_sum(acc);
         if (lane == 0) d.phi[r * K + c] = acc / sw;
     }
 }
@@ -283,19 +276,14 @@ int run_model(smcb_ctx *c, const smcb_online_desc &d) {
     M m;
     m.load(d.params);
     const size_t tab = TransUsesTable<M>::value ? kMathTabBytes : 0;
-    int rc;
     if (d.method == SMCB_ONLINE_PARIS) {
-        if ((rc = set_smem(k_paris<M>, tab)) != SMCB_OK) return rc;
+        SMCB_TRY(set_smem(k_paris<M>, tab));
         const int grid = (int)((d.N * d.Np + kSmBlock - 1) / kSmBlock);
-        k_paris<M><<<grid, kSmBlock, tab, c->stream>>>(m, d, key_of(d.seed ^ kOnlineSeedMix), c->math_tab);
-    } else {
-        if ((rc = set_smem(k_on2_weights<M>, tab)) != SMCB_OK) return rc;
-        const int grid = (int)((d.rows + kOnRows - 1) / kOnRows);
-        k_on2_weights<M><<<grid, kSmBlock, tab, c->stream>>>(m, d, c->math_tab);
+        return launch(c, k_paris<M>, grid, kSmBlock, tab, m, d, key_of(d.seed ^ kOnlineSeedMix), c->math_tab);
     }
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    SMCB_TRY(set_smem(k_on2_weights<M>, tab));
+    const int grid = (int)((d.rows + kOnRows - 1) / kOnRows);
+    return launch(c, k_on2_weights<M>, grid, kSmBlock, tab, m, d, c->math_tab);
 }
 
 }  // namespace
@@ -308,14 +296,10 @@ extern "C" int smcb_online_smooth(smcb_ctx *c, const smcb_online_desc *dp) {
         SMCB_REQUIRE(d.phi_prev && d.psi && d.phi && d.k >= 1, "smcb_online_smooth: NULL Phi or psi");
         if (d.method == SMCB_ONLINE_PHI_PARIS) {
             SMCB_REQUIRE(d.B && d.Np >= 1, "smcb_online_smooth: PHI_PARIS needs B and Np >= 1");
-            k_phi_paris<<<(int)((d.N + kBlock - 1) / kBlock), kBlock, 0, c->stream>>>(d);
-        } else {
-            SMCB_REQUIRE(d.omega && d.rows >= 1, "smcb_online_smooth: PHI_ON2 needs omega and rows >= 1");
-            k_phi_on2<<<(int)((d.rows * 32 + kBlock - 1) / kBlock), kBlock, 0, c->stream>>>(d);
+            return launch(c, k_phi_paris, (int)((d.N + kBlock - 1) / kBlock), kBlock, 0, d);
         }
-        c->launches++;
-        SMCB_CUDA(cudaGetLastError());
-        return SMCB_OK;
+        SMCB_REQUIRE(d.omega && d.rows >= 1, "smcb_online_smooth: PHI_ON2 needs omega and rows >= 1");
+        return launch(c, k_phi_on2, (int)((d.rows * 32 + kBlock - 1) / kBlock), kBlock, 0, d);
     }
     SMCB_REQUIRE(d.method == SMCB_ONLINE_PARIS || d.method == SMCB_ONLINE_ON2_W, "smcb_online_smooth: bad method %d",
                  (int)d.method);

@@ -21,8 +21,6 @@
 
 namespace smcb {
 
-constexpr uint32_t kPurposeTraj = 6;             // the uniform of the trajectory draw at step t
-
 // the uniform of the trajectory draw at step t: injected (ud[t]) or Philox
 __device__ __forceinline__ double traj_uniform(const Philox &key, int64_t t, const double *ud) {
     if (ud) return ud[t];
@@ -265,7 +263,7 @@ static int csmc_one(smcb_ctx *c, const smcb_csmc_desc &d, int64_t *out) {
         return SMCB_ENOSYS;
     }
     const size_t smem = csmc_smem(d.N);
-    SMCB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SMCB_TRY(set_smem(kern, smem));
     SMCB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kBatchBS, smem));
     if (nb < 1) {
         set_error("conditional SMC: the kernel does not fit on an SM of this device");
@@ -279,10 +277,7 @@ static int csmc_one(smcb_ctx *c, const smcb_csmc_desc &d, int64_t *out) {
         return SMCB_OK;
     }
     if (d.R == 0) return SMCB_OK;
-    kern<<<grid, kBatchBS, smem, c->stream>>>(d, c->math_tab);
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    return launch(c, kern, grid, kBatchBS, smem, d, c->math_tab);
 }
 
 static int csmc_dispatch(smcb_ctx *c, const smcb_csmc_desc *dp, int64_t *out) {

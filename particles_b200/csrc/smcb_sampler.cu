@@ -11,15 +11,9 @@
 // bound, and lower precision would change results (SURVEY.md section 8 row a23).
 #include "smcb_common.cuh"
 #include "smcb_math.cuh"
+#include "smcb_reduce.cuh"
 
 using namespace smcb;
-
-#define LAUNCHK(ctx, kern, grid, block, smem, ...)                               \
-    do {                                                                         \
-        kern<<<(grid), (block), (smem), (ctx)->stream>>>(__VA_ARGS__);           \
-        (ctx)->launches++;                                                       \
-        SMCB_CUDA(cudaGetLastError());                                           \
-    } while (0)
 
 namespace smcb {
 
@@ -150,7 +144,6 @@ __global__ void __launch_bounds__(kSampBlock) k_mh_accept(int64_t n, int d, doub
                                                          unsigned int *ticket, double *mean_acc,
                                                          uint8_t *accepted) {
     __shared__ double s_red[kSampBlock / 32];
-    __shared__ bool s_last;
     const int64_t i = (int64_t)blockIdx.x * kSampBlock + threadIdx.x;
     double pb = 0.0;
     if (i < n) {
@@ -169,25 +162,18 @@ __global__ void __launch_bounds__(kSampBlock) k_mh_accept(int64_t n, int d, doub
         }
         if (accepted) accepted[i] = (u < pb) ? 1 : 0;
     }
-    double acc = pb;
-#pragma unroll
-    for (int mask = 16; mask > 0; mask >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, mask);
+    const double acc = warp_sum(pb);
     if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = acc;
     __syncthreads();
     if (threadIdx.x == 0) {
         double t = 0.0;
         for (int w = 0; w < kSampBlock / 32; w++) t += s_red[w];
         partials[blockIdx.x] = t;
-        __threadfence();
-        s_last = (atomicInc(ticket, gridDim.x - 1) == gridDim.x - 1);
     }
-    __syncthreads();
-    if (s_last && threadIdx.x == 0) {
-        __threadfence();
-        double t = 0.0;
-        for (unsigned int b = 0; b < gridDim.x; b++) t += ((volatile double *)partials)[b];
-        mean_acc[0] = t / (double)n;
-    }
+    if (!last_block(ticket) || threadIdx.x != 0) return;
+    double t = 0.0;
+    for (unsigned int b = 0; b < gridDim.x; b++) t += ((volatile double *)partials)[b];
+    mean_acc[0] = t / (double)n;
 }
 
 // ---------------------------------------------------------------------------
@@ -328,14 +314,13 @@ static int launch_wf(smcb_ctx *c, int64_t M, int d, int P, const double *theta0,
     int64_t tile_rows = (int64_t)((budget - fixed) / (D * sizeof(double)));
     if (tile_rows > n_data) tile_rows = n_data;
     const size_t smem = fixed + (size_t)tile_rows * D * sizeof(double);
-    SMCB_CUDA(cudaFuncSetAttribute(k_logistic_wf_move<D, FLOOR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SMCB_TRY(set_smem(k_logistic_wf_move<D, FLOOR>, smem));
     const int chains_per_block = kWfBlock / kWfLanes;
     const int grid = (int)((M + chains_per_block - 1) / chains_per_block);
     const uint64_t call = (z_in && u_in) ? 0 : c->api_counter++;
-    LAUNCHK(c, (k_logistic_wf_move<D, FLOOR>), grid, kWfBlock, smem, M, d, P, theta0, lprior0, llik0, lpost0, data, n_data,
-            (int)tile_rows, s, lognorm, epn, L, key_of(c->seed), call, z_in, u_in, theta_out, lprior_out, llik_out,
-            lpost_out, pb_out);
-    return SMCB_OK;
+    return launch(c, k_logistic_wf_move<D, FLOOR>, grid, kWfBlock, smem, M, d, P, theta0, lprior0, llik0, lpost0, data,
+                  n_data, (int)tile_rows, s, lognorm, epn, L, key_of(c->seed), call, z_in, u_in, theta_out, lprior_out,
+                  llik_out, lpost_out, pb_out);
 }
 
 template <bool FLOOR>
@@ -393,9 +378,8 @@ static int launch_target(smcb_ctx *c, const double *theta, int64_t n, int d, con
                          double *lpost) {
     const int64_t pairs = (n + 1) / 2;
     const int grid = (int)((pairs + kSampBlock - 1) / kSampBlock);
-    LAUNCHK(c, (k_logistic_target<D, FLOOR>), grid, kSampBlock, 0, theta, n, d, data, n_data, s, lognorm, epn, lprior,
-            llik, lpost);
-    return SMCB_OK;
+    return launch(c, k_logistic_target<D, FLOOR>, grid, kSampBlock, 0, theta, n, d, data, n_data, s, lognorm, epn,
+                  lprior, llik, lpost);
 }
 
 template <bool FLOOR>
@@ -439,9 +423,8 @@ extern "C" int smcb_rw_propose(smcb_ctx *c, const double *theta, int64_t n, int 
     SMCB_REQUIRE(n >= 1 && d >= 1 && d <= 32, "smcb_rw_propose: need 1 <= d <= 32");
     const uint64_t call = z_in ? 0 : c->api_counter++;
     const int grid = (int)((n + kSampBlock - 1) / kSampBlock);
-    LAUNCHK(c, k_rw_propose, grid, kSampBlock, (size_t)d * d * sizeof(double), theta, n, L_dev, d,
-            key_of(c->seed), call, z_in, prop);
-    return SMCB_OK;
+    return launch(c, k_rw_propose, grid, kSampBlock, (size_t)d * d * sizeof(double), theta, n, L_dev, d,
+                  key_of(c->seed), call, z_in, prop);
 }
 
 // ArrayMetropolis.step accept / copyto (smc_samplers.py:605-611); mean_acc: device scalar; accepted: NULL or (n)
@@ -455,9 +438,8 @@ extern "C" int smcb_mh_accept_flags(smcb_ctx *c, int64_t n, int d, double *theta
     const int grid = (int)((n + kSampBlock - 1) / kSampBlock);
     SMCB_REQUIRE((size_t)grid <= kWsPartials, "smcb_mh_accept: too many particles for the workspace");
     const uint64_t call = u_in ? 0 : c->api_counter++;
-    LAUNCHK(c, k_mh_accept, grid, kSampBlock, 0, n, d, theta, lprior, llik, lpost, theta_p, lprior_p, llik_p,
-            lpost_p, key_of(c->seed), call, u_in, c->ws, c->counters + 2, mean_acc, accepted);
-    return SMCB_OK;
+    return launch(c, k_mh_accept, grid, kSampBlock, 0, n, d, theta, lprior, llik, lpost, theta_p, lprior_p, llik_p,
+                  lpost_p, key_of(c->seed), call, u_in, c->ws, c->counters + kTicketMhAccept, mean_acc, accepted);
 }
 
 extern "C" int smcb_mh_accept(smcb_ctx *c, int64_t n, int d, double *theta, double *lprior, double *llik,
@@ -482,25 +464,20 @@ constexpr int kCtlGrid = kSMs * 2;
 __global__ void __launch_bounds__(kCtlBlock) k_ctl_max(const double *__restrict__ v, int64_t n, double *partials,
                                                       unsigned int *ticket, double *out) {
     __shared__ double s[kCtlBlock / 32];
-    __shared__ bool last;
     double m = -CUDART_INF;
     for (int64_t i = (int64_t)blockIdx.x * kCtlBlock + threadIdx.x; i < n; i += (int64_t)gridDim.x * kCtlBlock)
         m = fmax(m, v[i]);
-    for (int k = 16; k > 0; k >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, k));
+    m = warp_max(m);
     if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = m;
     __syncthreads();
     if (threadIdx.x == 0) {
         for (int w = 1; w < kCtlBlock / 32; w++) m = fmax(m, s[w]);
         partials[blockIdx.x] = m;
-        __threadfence();
-        last = atomicInc(ticket, gridDim.x - 1) == gridDim.x - 1;
     }
-    __syncthreads();
-    if (last && threadIdx.x == 0) {
-        double r = -CUDART_INF;
-        for (unsigned int b = 0; b < gridDim.x; b++) r = fmax(r, reinterpret_cast<volatile double *>(partials)[b]);
-        out[0] = r;
-    }
+    if (!last_block(ticket) || threadIdx.x != 0) return;
+    double r = -CUDART_INF;
+    for (unsigned int b = 0; b < gridDim.x; b++) r = fmax(r, reinterpret_cast<volatile double *>(partials)[b]);
+    out[0] = r;
 }
 
 // one pass of the root-find of next_annealing_epn (smc_samplers.py:876-895): ESS(delta * lw) at the kRootWays
@@ -510,7 +487,6 @@ __global__ void __launch_bounds__(kCtlBlock) k_ctl_root_pass(const double *__res
                                                             double *state, double *partials, unsigned int *ticket,
                                                             int final_pass, double *raw_out) {
     __shared__ double s_red[kCtlBlock / 32][2 * kRootWays];
-    __shared__ bool last;
     const double lo = state[0], hi = state[1], M = state[2];
     if (state[3] != 0.0) return;                                   // already decided (delta = full step)
     double dj[kRootWays], s[kRootWays], q[kRootWays];
@@ -527,10 +503,8 @@ __global__ void __launch_bounds__(kCtlBlock) k_ctl_root_pass(const double *__res
     }
 #pragma unroll
     for (int j = 0; j < kRootWays; j++) {
-        for (int k = 16; k > 0; k >>= 1) {
-            s[j] += __shfl_xor_sync(0xffffffffu, s[j], k);
-            q[j] += __shfl_xor_sync(0xffffffffu, q[j], k);
-        }
+        s[j] = warp_sum(s[j]);
+        q[j] = warp_sum(q[j]);
         if ((threadIdx.x & 31) == 0) { s_red[threadIdx.x >> 5][2 * j] = s[j]; s_red[threadIdx.x >> 5][2 * j + 1] = q[j]; }
     }
     __syncthreads();
@@ -539,12 +513,7 @@ __global__ void __launch_bounds__(kCtlBlock) k_ctl_root_pass(const double *__res
         for (int w = 0; w < kCtlBlock / 32; w++) v += s_red[w][threadIdx.x];
         partials[(size_t)blockIdx.x * 2 * kRootWays + threadIdx.x] = v;
     }
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) last = atomicInc(ticket, gridDim.x - 1) == gridDim.x - 1;
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
+    if (!last_block(ticket)) return;
     __shared__ double tot[2 * kRootWays];
     if (threadIdx.x < 2 * kRootWays) {                             // fixed block order: deterministic
         double v = 0.0;
@@ -616,7 +585,6 @@ __global__ void __launch_bounds__(kCtlBlock) k_ctl_wcov(const double *__restrict
                                                        int64_t n, int d, double *work /* [0..d) mean | d x d cov */,
                                                        double *partials, unsigned int *ticket, double scale,
                                                        double *L_out, const double *mean) {
-    __shared__ bool last;
     extern __shared__ double s_acc[];                              // (kCtlBlock/32) x nvals
     const int nvals = (PASS == 0) ? d + 1 : d * (d + 1) / 2;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -656,12 +624,7 @@ __global__ void __launch_bounds__(kCtlBlock) k_ctl_wcov(const double *__restrict
         for (int w2 = 0; w2 < kCtlBlock / 32; w2++) t += s_acc[w2 * nvals + v];
         partials[(size_t)blockIdx.x * nvals + v] = t;
     }
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) last = atomicInc(ticket, gridDim.x - 1) == gridDim.x - 1;
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
+    if (!last_block(ticket)) return;
     double *tot = s_acc;
     for (int v = threadIdx.x; v < nvals; v += kCtlBlock) {
         double t = 0.0;
@@ -694,14 +657,12 @@ extern "C" int smcb_next_annealing_epn(smcb_ctx *c, const double *lw, int64_t n,
     const double init[5] = {0.0, 1.0 - epn, 0.0, 0.0, 0.0};
     SMCB_CUDA(cudaMemcpyAsync(state, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
     const int grid = (int)((n + kCtlBlock - 1) / kCtlBlock < kCtlGrid ? (n + kCtlBlock - 1) / kCtlBlock : kCtlGrid);
-    LAUNCHK(c, k_ctl_max, grid, kCtlBlock, 0, lw, n, partials, c->counters + 8, state + 2);
+    SMCB_TRY(launch(c, k_ctl_max, grid, kCtlBlock, 0, lw, n, partials, c->counters + kTicketCtlMax, state + 2));
     for (int p = 0; p < kRootPasses; p++)
-        LAUNCHK(c, k_ctl_root_pass, grid, kCtlBlock, 0, lw, n, alpha * (double)n, state, partials, c->counters + 9,
-                (p == kRootPasses - 1 ? 1 : 0) | (p == 0 ? 2 : 0), (double *)nullptr);
-    k_ctl_root_finish<<<1, 1, 0, c->stream>>>(state, epn, out_dev);     // result = epn + delta
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+        SMCB_TRY(launch(c, k_ctl_root_pass, grid, kCtlBlock, 0, lw, n, alpha * (double)n, state, partials,
+                        c->counters + kTicketCtlRoot, (p == kRootPasses - 1 ? 1 : 0) | (p == 0 ? 2 : 0),
+                        (double *)nullptr));
+    return launch(c, k_ctl_root_finish, 1, 1, 0, state, epn, out_dev);     // result = epn + delta
 }
 
 // ArrayRandomWalk.calibrate (smc_samplers.py:617-622): L = scale * chol(wcov(W, theta)) on the device
@@ -713,11 +674,10 @@ extern "C" int smcb_rw_calibrate(smcb_ctx *c, const double *W, const double *the
     double *partials = c->ws + 1024;
     const int grid = (int)((n + 7) / 8 < kCtlGrid ? (n + 7) / 8 : kCtlGrid);
     const int nv0 = d + 1, nv1 = d * (d + 1) / 2;
-    LAUNCHK(c, (k_ctl_wcov<0, true>), grid, kCtlBlock, (kCtlBlock / 32) * (nv0 > 32 ? nv0 : 32) * sizeof(double), W, theta, n, d,
-            work, partials, c->counters + 10, scale, L_out, (const double *)nullptr);
-    LAUNCHK(c, (k_ctl_wcov<1, true>), grid, kCtlBlock, (kCtlBlock / 32) * nv1 * sizeof(double), W, theta, n, d, work, partials,
-            c->counters + 11, scale, L_out, (const double *)work);
-    return SMCB_OK;
+    SMCB_TRY(launch(c, k_ctl_wcov<0, true>, grid, kCtlBlock, (kCtlBlock / 32) * (nv0 > 32 ? nv0 : 32) * sizeof(double), W,
+                    theta, n, d, work, partials, c->counters + kTicketCtlWcov0, scale, L_out, (const double *)nullptr));
+    return launch(c, k_ctl_wcov<1, true>, grid, kCtlBlock, (kCtlBlock / 32) * nv1 * sizeof(double), W, theta, n, d, work,
+                  partials, c->counters + kTicketCtlWcov1, scale, L_out, (const double *)work);
 }
 
 // the same in pieces for a run sharded over ranks (the caller all-reduces between them):
@@ -730,19 +690,17 @@ extern "C" int smcb_wcov_sums(smcb_ctx *c, const double *W, const double *theta,
     const int grid = (int)((n + 7) / 8 < kCtlGrid ? (n + 7) / 8 : kCtlGrid);
     const int nv0 = d + 1, nv1 = d * (d + 1) / 2;
     if (mean_dev == nullptr)
-        LAUNCHK(c, (k_ctl_wcov<0, false>), grid, kCtlBlock, (kCtlBlock / 32) * (nv0 > 32 ? nv0 : 32) * sizeof(double), W, theta,
-                n, d, out_dev, partials, c->counters + 10, 1.0, (double *)nullptr, (const double *)nullptr);
-    else
-        LAUNCHK(c, (k_ctl_wcov<1, false>), grid, kCtlBlock, (kCtlBlock / 32) * nv1 * sizeof(double), W, theta, n, d, out_dev,
-                partials, c->counters + 11, 1.0, (double *)nullptr, mean_dev);
-    return SMCB_OK;
+        return launch(c, k_ctl_wcov<0, false>, grid, kCtlBlock, (kCtlBlock / 32) * (nv0 > 32 ? nv0 : 32) * sizeof(double),
+                      W, theta, n, d, out_dev, partials, c->counters + kTicketCtlWcov0, 1.0, (double *)nullptr,
+                      (const double *)nullptr);
+    return launch(c, k_ctl_wcov<1, false>, grid, kCtlBlock, (kCtlBlock / 32) * nv1 * sizeof(double), W, theta, n, d,
+                  out_dev, partials, c->counters + kTicketCtlWcov1, 1.0, (double *)nullptr, mean_dev);
 }
 
 extern "C" int smcb_chol_from_sums(smcb_ctx *c, const double *tri_dev, const double *sw_dev, int d, double scale,
                                    double *L_out) {
     SMCB_REQUIRE(c && tri_dev && sw_dev && L_out && d >= 1 && d <= 20, "smcb_chol_from_sums: bad argument");
-    LAUNCHK(c, k_ctl_chol, 1, 32, 0, tri_dev, sw_dev, d, scale, c->ws, L_out);
-    return SMCB_OK;
+    return launch(c, k_ctl_chol, 1, 32, 0, tri_dev, sw_dev, d, scale, c->ws, L_out);
 }
 
 // one pass of the root-find's ESS grid without the bracket update (sharded runs): out32_dev = {s_j, q_j} for the 16
@@ -756,8 +714,8 @@ extern "C" int smcb_essl_grid(smcb_ctx *c, const double *lw, int64_t n, double l
     SMCB_CUDA(cudaMemcpyAsync(state, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
     SMCB_CUDA(cudaMemcpyAsync(state + 2, max_dev, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
     const int grid = (int)((n + kCtlBlock - 1) / kCtlBlock < kCtlGrid ? (n + kCtlBlock - 1) / kCtlBlock : kCtlGrid);
-    LAUNCHK(c, k_ctl_root_pass, grid, kCtlBlock, 0, lw, n, 0.0, state, partials, c->counters + 9, 0, out32_dev);
-    return SMCB_OK;
+    return launch(c, k_ctl_root_pass, grid, kCtlBlock, 0, lw, n, 0.0, state, partials, c->counters + kTicketCtlRoot, 0,
+                  out32_dev);
 }
 
 // ---------------------------------------------------------------------------
@@ -838,13 +796,8 @@ static int launch_logpyt(smcb_ctx *c, const double *theta, int64_t n, int d, con
                          int64_t K, int commit, double *lw, double *lpost, double *llik, double *scratch) {
     const int64_t pairs = (n + 1) / 2;
     const int grid = (int)((pairs + kSampBlock - 1) / kSampBlock);
-    if (commit)
-        LAUNCHK(c, (k_logistic_logpyt<D, true>), grid, kSampBlock, 0, theta, n, d, data, r0, K, lw, lpost, llik,
-                scratch);
-    else
-        LAUNCHK(c, (k_logistic_logpyt<D, false>), grid, kSampBlock, 0, theta, n, d, data, r0, K, lw, lpost, llik,
-                scratch);
-    return SMCB_OK;
+    return launch(c, commit ? k_logistic_logpyt<D, true> : k_logistic_logpyt<D, false>, grid, kSampBlock, 0, theta, n,
+                  d, data, r0, K, lw, lpost, llik, scratch);
 }
 
 // IBIS.logG (smc_samplers.py:773-776) for the logistic-regression model over the rows [r0, r0 + K) of data

@@ -241,7 +241,7 @@ __global__ void __launch_bounds__(kSmBlock) k_bs_reject(M m, smcb_smooth_desc d,
             }
         }
         // acceptance statistics: integer sums, one atomic pair per warp (order-independent -> deterministic)
-        const long long na = warp_sum((live && acc) ? 1 : 0), np = warp_sum(nprop);
+        const long long na = warp_sum((live && acc) ? 1LL : 0LL), np = warp_sum(nprop);
         if (lane == 0) {
             atomicAdd(reinterpret_cast<unsigned long long *>(d.counts + 2 * t), (unsigned long long)na);
             atomicAdd(reinterpret_cast<unsigned long long *>(d.counts + 2 * t + 1), (unsigned long long)np);
@@ -290,22 +290,18 @@ int run_model(smcb_ctx *c, const smcb_smooth_desc &d) {
     const uint64_t call = c->api_counter++;
     const int grid = (int)((d.M + kSmBlock - 1) / kSmBlock);
     const size_t tab = TransUsesTable<M>::value ? kMathTabBytes : 0;
-    int rc;
     if (d.method == SMCB_SMOOTH_ON2) {
         const size_t smem = kMathTabBytes + (size_t)(M::D + 1) * kSmBlock * sizeof(double);
-        if ((rc = set_smem(k_bs_on2<M>, smem)) != SMCB_OK) return rc;
-        k_bs_on2<M><<<grid, kSmBlock, smem, c->stream>>>(m, d, key, call, c->math_tab);
-    } else if (d.method == SMCB_SMOOTH_MCMC) {
-        if ((rc = set_smem(k_bs_mcmc<M>, tab)) != SMCB_OK) return rc;
-        k_bs_mcmc<M><<<grid, kSmBlock, tab, c->stream>>>(m, d, key, call, c->math_tab);
-    } else {
-        if ((rc = set_smem(k_bs_reject<M>, tab)) != SMCB_OK) return rc;
-        SMCB_CUDA(cudaMemsetAsync(d.counts, 0, (size_t)(d.T - 1) * 2 * sizeof(int64_t), c->stream));
-        k_bs_reject<M><<<grid, kSmBlock, tab, c->stream>>>(m, d, key, call, c->math_tab);
+        SMCB_TRY(set_smem(k_bs_on2<M>, smem));
+        return launch(c, k_bs_on2<M>, grid, kSmBlock, smem, m, d, key, call, c->math_tab);
     }
-    c->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    if (d.method == SMCB_SMOOTH_MCMC) {
+        SMCB_TRY(set_smem(k_bs_mcmc<M>, tab));
+        return launch(c, k_bs_mcmc<M>, grid, kSmBlock, tab, m, d, key, call, c->math_tab);
+    }
+    SMCB_TRY(set_smem(k_bs_reject<M>, tab));
+    SMCB_CUDA(cudaMemsetAsync(d.counts, 0, (size_t)(d.T - 1) * 2 * sizeof(int64_t), c->stream));
+    return launch(c, k_bs_reject<M>, grid, kSmBlock, tab, m, d, key, call, c->math_tab);
 }
 
 }  // namespace
@@ -317,12 +313,7 @@ extern "C" int smcb_backward_sample(smcb_ctx *c, const smcb_smooth_desc *dp) {
                  "smcb_backward_sample: bad sizes T=%lld N=%lld M=%lld", (long long)d.T, (long long)d.N,
                  (long long)d.M);
     SMCB_REQUIRE(d.X && d.idx && d.paths && d.dim >= 1, "smcb_backward_sample: NULL history or output");
-    if (d.method == SMCB_SMOOTH_GATHER) {
-        k_bs_gather<<<grid_for(d.T * d.M * d.dim, kBlock * 4), kBlock, 0, c->stream>>>(d);
-        c->launches++;
-        SMCB_CUDA(cudaGetLastError());
-        return SMCB_OK;
-    }
+    if (d.method == SMCB_SMOOTH_GATHER) return launch(c, k_bs_gather, grid_for(d.T * d.M * d.dim, kBlock * 4), kBlock, 0, d);
     SMCB_REQUIRE(d.method >= SMCB_SMOOTH_ON2 && d.method <= SMCB_SMOOTH_REJECT, "smcb_backward_sample: bad method %d",
                  (int)d.method);
     SMCB_REQUIRE(d.lw && d.idx_T, "smcb_backward_sample: NULL log-weights or final indices");

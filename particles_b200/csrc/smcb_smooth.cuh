@@ -1,6 +1,6 @@
 // smcb_smooth.cuh -- device pieces shared by the backward samplers (smcb_smooth.cu) and the on-line smoothers
 // (smcb_online.cu): Philox uniforms of a draw, inverse-CDF multinomial draw, online log-sum-exp, the warp-cooperative
-// exact draw and one rejection trial; on the host, the shared-memory attribute of a launch.
+// exact draw and one rejection trial.
 //
 // The history-reading helpers are templated on the descriptor.  A descriptor `d` provides the pointer tables
 // d.X[t] and d.lw[t], the element strides d.x_stride_n / d.x_stride_c, the sizes d.N (particles at t), d.M (draws)
@@ -17,13 +17,11 @@
 #include "smcb_common.cuh"
 #include "smcb_math.cuh"
 #include "smcb_models.cuh"
+#include "smcb_reduce.cuh"
 
 namespace smcb {
 
 constexpr int kSmBlock = 256;                  // threads per CTA; ON2: trajectories per CTA = particles per tile
-constexpr uint32_t kPurposeSmooth = 4;         // proposal + acceptance uniforms of trial `trial`
-constexpr uint32_t kPurposeSmoothExact = 5;    // the uniform of an exact O(N) draw
-constexpr unsigned kFull = 0xffffffffu;
 
 __device__ __forceinline__ void smooth_uniforms(const Philox &key, uint64_t call, int64_t m, int64_t t, uint32_t trial,
                                                 uint32_t purpose, double &u0, double &u1) {
@@ -76,6 +74,15 @@ __device__ __forceinline__ void lse_merge(double &mx, double &s, double mo, doub
     }
 }
 
+// lse_merge of the lanes' (mx, s) by the xor butterfly, strides 16 -> 1: every lane gets the same bits
+__device__ __forceinline__ void warp_lse_merge(double &mx, double &s) {
+#pragma unroll
+    for (int mask = 16; mask > 0; mask >>= 1) {
+        const double mo = __shfl_xor_sync(kFull, mx, mask), so = __shfl_xor_sync(kFull, s, mask);
+        lse_merge(mx, s, mo, so);
+    }
+}
+
 template <class M>
 __device__ __forceinline__ void stage_tables(const double *tab, uint64_t *bar, bool needed) {
     if (!needed) return;
@@ -101,11 +108,7 @@ __device__ int64_t warp_exact_draw(const M &m, const TransDensity<M> &td, const 
     };
     double mx = -CUDART_INF, s = 0.0;
     for (int64_t n = lane; n < N; n += 32) lse_add<false>(mx, s, value(n));
-#pragma unroll
-    for (int mask = 16; mask > 0; mask >>= 1) {
-        const double mo = __shfl_xor_sync(kFull, mx, mask), so = __shfl_xor_sync(kFull, s, mask);
-        lse_merge(mx, s, mo, so);
-    }
+    warp_lse_merge(mx, s);
     const double target = u * s;
     double c = 0.0;
     int64_t last = -1;
@@ -134,12 +137,6 @@ __device__ int64_t warp_exact_draw(const M &m, const TransDensity<M> &td, const 
     return last >= 0 ? last : 0;
 }
 
-__device__ __forceinline__ long long warp_sum(long long v) {
-#pragma unroll
-    for (int mask = 16; mask > 0; mask >>= 1) v += __shfl_xor_sync(kFull, v, mask);
-    return v;
-}
-
 // trial `trial` of draw jj at time t: proposal (returned in prop) and acceptance test (smoothing.py:405-410)
 template <class M, class Desc>
 __device__ __forceinline__ bool reject_trial(const M &m, const TransDensity<M> &td, const Desc &d,
@@ -165,12 +162,5 @@ __device__ __forceinline__ bool reject_trial(const M &m, const TransDensity<M> &
 
 // trials each lane runs on its own before the warp serves the lanes still rejected together
 constexpr int64_t kSoloTrials = 4;
-
-// host: lets launches of `kern` use `bytes` of dynamic shared memory
-template <class K>
-int set_smem(K kern, size_t bytes) {
-    SMCB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    return SMCB_OK;
-}
 
 }  // namespace smcb

@@ -2093,10 +2093,7 @@ template <class M, int FK>
 static int launch_init_t(smcb_filter *f) {
     M model;
     model.load(f->desc.params);
-    k_init<M, FK><<<f->grid_move, f->block_size, kMathTabBytes, f->ctx->stream>>>(model, f->args);
-    f->ctx->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    return launch(f->ctx, k_init<M, FK>, f->grid_move, f->block_size, kMathTabBytes, model, f->args);
 }
 
 template <int FK>
@@ -2107,10 +2104,7 @@ static int launch_tail_t(smcb_filter *f) {
 
 template <int FK>
 static int launch_publish_t(smcb_filter *f) {
-    k_publish<FkTraits<FK>::apf><<<1, kTailBlock, 0, f->ctx->stream>>>(f->args, (long long)(f->t_host - 1));
-    f->ctx->launches++;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    return launch(f->ctx, k_publish<FkTraits<FK>::apf>, 1, kTailBlock, 0, f->args, (long long)(f->t_host - 1));
 }
 
 template <class M, int FK, int SCHEME>
@@ -2123,9 +2117,8 @@ static int bind_one(smcb_filter *f) {
     f->dyn_smem = StepCfg<M>::dyn_smem;
     f->slab_doubles = StepCfg<M>::kSlabDoubles;
     f->pairs_per_iteration = 32 * StepCfg<M>::kU;
-    SMCB_CUDA(cudaFuncSetAttribute(k_step<M, FK, SCHEME>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)StepCfg<M>::dyn_smem));
-    SMCB_CUDA(cudaFuncSetAttribute(k_init<M, FK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMathTabBytes));
+    SMCB_TRY(set_smem(k_step<M, FK, SCHEME>, StepCfg<M>::dyn_smem));
+    SMCB_TRY(set_smem(k_init<M, FK>, kMathTabBytes));
     int nb = 0;
     SMCB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_step<M, FK, SCHEME>, StepCfg<M>::BS,
                                                             StepCfg<M>::dyn_smem));

@@ -140,19 +140,14 @@ int run_model(smcb_ctx *c, const smcb_twofilter_desc &d) {
         M m;
         m.load(d.params);
         const size_t tab = TransUsesTable<M>::value ? kMathTabBytes : 0;
-        int rc;
         if (d.method == SMCB_TF_ON2_ROWS) {
-            if ((rc = set_smem(k_tf_on2_rows<M>, tab)) != SMCB_OK) return rc;
+            SMCB_TRY(set_smem(k_tf_on2_rows<M>, tab));
             const int grid = (int)((d.rows + kTfRows - 1) / kTfRows);
-            k_tf_on2_rows<M><<<grid, kSmBlock, tab, c->stream>>>(m, d, c->math_tab);
-        } else {
-            if ((rc = set_smem(k_tf_on_logw<M>, tab)) != SMCB_OK) return rc;
-            const int grid = (int)((d.M + kSmBlock - 1) / kSmBlock);
-            k_tf_on_logw<M><<<grid, kSmBlock, tab, c->stream>>>(m, d, c->math_tab);
+            return launch(c, k_tf_on2_rows<M>, grid, kSmBlock, tab, m, d, c->math_tab);
         }
-        c->launches++;
-        SMCB_CUDA(cudaGetLastError());
-        return SMCB_OK;
+        SMCB_TRY(set_smem(k_tf_on_logw<M>, tab));
+        const int grid = (int)((d.M + kSmBlock - 1) / kSmBlock);
+        return launch(c, k_tf_on_logw<M>, grid, kSmBlock, tab, m, d, c->math_tab);
     }
 }
 

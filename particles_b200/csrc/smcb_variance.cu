@@ -224,10 +224,7 @@ extern "C" int smcb_variance(smcb_ctx *c, const smcb_variance_desc *dp) {
     SMCB_REQUIRE(d.B[0] && (!d.parity || d.B[1]), "smcb_variance: NULL Eve rows");
     if (d.method == SMCB_VAR_EVE) {
         SMCB_REQUIRE(d.parity && d.A, "smcb_variance: EVE needs the parity word and the ancestors");
-        k_var_eve<<<grid_for(d.N, kBlock), kBlock, 0, c->stream>>>(d);
-        c->launches++;
-        SMCB_CUDA(cudaGetLastError());
-        return SMCB_OK;
+        return launch(c, k_var_eve, grid_for(d.N, kBlock), kBlock, 0, d);
     }
     SMCB_REQUIRE(d.method == SMCB_VAR_SUMS, "smcb_variance: bad method %d", (int)d.method);
     SMCB_REQUIRE(d.mode == SMCB_VAR_CENTRED || d.mode == SMCB_VAR_WEIGHTS, "smcb_variance: bad mode %d", (int)d.mode);
@@ -240,11 +237,8 @@ extern "C" int smcb_variance(smcb_ctx *c, const smcb_variance_desc *dp) {
     const int64_t nch = n_chunks(d.N);
     SMCB_REQUIRE(nch <= 0x7fffffffLL, "smcb_variance: N too large");
     double *stats = d.scratch, *rec1 = stats + 3 * d.k, *rec2 = rec1 + kVarRec1 * d.k * nch;
-    k_var_p1<<<dim3((unsigned)nch, (unsigned)d.k), kVarThreads, 0, c->stream>>>(d, rec1);
-    k_var_f1<<<1, kVarFin, 0, c->stream>>>(d, rec1, nch, stats);
-    k_var_p2<<<dim3((unsigned)nch, (unsigned)(d.L * d.k)), kVarThreads, 0, c->stream>>>(d, stats, rec2);
-    k_var_f2<<<1, kVarFin, 0, c->stream>>>(d, rec2, nch);
-    c->launches += 4;
-    SMCB_CUDA(cudaGetLastError());
-    return SMCB_OK;
+    SMCB_TRY(launch(c, k_var_p1, dim3((unsigned)nch, (unsigned)d.k), kVarThreads, 0, d, rec1));
+    SMCB_TRY(launch(c, k_var_f1, 1, kVarFin, 0, d, rec1, nch, stats));
+    SMCB_TRY(launch(c, k_var_p2, dim3((unsigned)nch, (unsigned)(d.L * d.k)), kVarThreads, 0, d, stats, rec2));
+    return launch(c, k_var_f2, 1, kVarFin, 0, d, rec2, nch);
 }
