@@ -12,6 +12,8 @@ SO_PATH = os.environ.get("SMCB_LIB") or os.path.join(HERE, "libsmcb.so")   # SMC
 SMCB_MAX_PARAMS = 256
 SUMMARY_STRIDE = 4
 
+OK, EINVAL, ECUDA, ENOSYS = 0, -1, -2, -3   # return codes of every entry point
+
 RS_CODES = {"multinomial": 0, "stratified": 1, "systematic": 2, "residual": 3, "ssp": 4}
 FUSED_SCHEMES = ("multinomial", "stratified", "systematic")     # schemes built into the fused step kernel
 FK_BOOTSTRAP, FK_GUIDED, FK_APF, FK_AUXBOOT = 0, 1, 2, 3
@@ -22,7 +24,10 @@ LSE_SUM, LSE_MEAN, LSE_ESSL = 0, 1, 2
 c_dp = C.c_void_p  # device pointers travel as integers
 
 
+# Every descriptor has __slots__ = (): a misspelt field name raises AttributeError instead of creating a Python
+# attribute that the library never reads.
 class FilterDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("model", C.c_int32), ("fk", C.c_int32), ("scheme", C.c_int32), ("dim", C.c_int32),
         ("dy", C.c_int32), ("n_params", C.c_int32), ("world", C.c_int32), ("rank", C.c_int32),
@@ -42,6 +47,7 @@ SMOOTH_ON2, SMOOTH_MCMC, SMOOTH_REJECT, SMOOTH_GATHER = 0, 1, 2, 3
 
 
 class SmoothDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("method", C.c_int32), ("model", C.c_int32), ("dim", C.c_int32), ("n_params", C.c_int32),
         ("T", C.c_int64), ("N", C.c_int64), ("M", C.c_int64), ("nsteps", C.c_int64), ("max_trials", C.c_int64),
@@ -57,6 +63,7 @@ ONLINE_PARIS, ONLINE_ON2_W, ONLINE_PHI_PARIS, ONLINE_PHI_ON2 = 0, 1, 2, 3
 
 
 class OnlineDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("method", C.c_int32), ("model", C.c_int32), ("dim", C.c_int32), ("n_params", C.c_int32),
         ("t", C.c_int64), ("N", C.c_int64), ("Np", C.c_int64), ("max_trials", C.c_int64),
@@ -72,6 +79,7 @@ TF_ON2_ROWS, TF_ON_LOGW = 0, 1
 
 
 class TwoFilterDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("method", C.c_int32), ("model", C.c_int32), ("dim", C.c_int32), ("n_params", C.c_int32),
         ("t", C.c_int64), ("N", C.c_int64), ("Ninfo", C.c_int64), ("row0", C.c_int64), ("rows", C.c_int64),
@@ -87,6 +95,7 @@ VAR_CENTRED, VAR_WEIGHTS = 0, 1
 
 
 class VarDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("method", C.c_int32), ("mode", C.c_int32), ("lin_w", C.c_int32), ("rs_host", C.c_int32),
         ("N", C.c_int64), ("k", C.c_int64), ("L", C.c_int64),
@@ -101,6 +110,7 @@ BATCH_TIERS = {"auto": BATCH_AUTO, "resident": BATCH_RESIDENT, "streaming": BATC
 
 
 class BatchDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("model", C.c_int32), ("fk", C.c_int32), ("scheme", C.c_int32), ("dim", C.c_int32),
         ("dy", C.c_int32), ("n_params", C.c_int32), ("tier", C.c_int32), ("reserved0", C.c_int32),
@@ -115,6 +125,7 @@ BANK_STATE = 8
 
 
 class BankDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("model", C.c_int32), ("fk", C.c_int32), ("scheme", C.c_int32), ("tier", C.c_int32),
         ("n_params", C.c_int32), ("restart", C.c_int32),
@@ -130,6 +141,7 @@ CSMC_GENEALOGY, CSMC_BACKWARD = 0, 1
 
 
 class CsmcDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("model", C.c_int32), ("fk", C.c_int32), ("n_params", C.c_int32), ("draw", C.c_int32),
         ("pin", C.c_int32), ("reserved0", C.c_int32),
@@ -146,6 +158,7 @@ HMM_MAX_K = 128
 
 
 class HmmDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("method", C.c_int32), ("K", C.c_int32), ("B", C.c_int64), ("ld", C.c_int64),
         ("t0", C.c_int64), ("t1", C.c_int64), ("N", C.c_int64), ("seed", C.c_uint64),
@@ -160,6 +173,7 @@ KALMAN_MAX_D = 32
 
 
 class KalmanDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("method", C.c_int32), ("dx", C.c_int32), ("dy", C.c_int32), ("pad_", C.c_int32),
         ("B", C.c_int64), ("ld", C.c_int64), ("t0", C.c_int64), ("t1", C.c_int64),
@@ -172,6 +186,7 @@ class KalmanDesc(C.Structure):
 
 
 class VsDesc(C.Structure):
+    __slots__ = ()
     _fields_ = [
         ("p", C.c_int32), ("use_ldet", C.c_int32), ("xtx", c_dp), ("xty", c_dp), ("vm2", C.c_double),
         ("coef_len", C.c_double), ("coef_log", C.c_double), ("coef_in_log", C.c_double), ("gw", C.c_double),
@@ -294,11 +309,11 @@ def load():
 
 
 def check(rc):
-    if rc == 0:
+    if rc == OK:
         return
     msg = load().smcb_last_error().decode()
-    if rc == -1:
+    if rc == EINVAL:
         raise ValueError(msg)
-    if rc == -3:
+    if rc == ENOSYS:
         raise NotImplementedError(msg)
     raise SmcbError(msg)

@@ -1,35 +1,17 @@
 """SMC samplers on binary spaces, the parts that need no device: the NumPy oracle against the live reference's
-golden vectors (tests/golden/golden_binary.npz), the model descriptor against include/smcb.h, the host-side
-NestedLogistic.fit against the reference's coefficients, and the refusals of the public surface."""
-import ctypes as C
+golden vectors (tests/golden/golden_binary.npz), the host-side NestedLogistic.fit against the reference's
+coefficients, and the refusals of the public surface."""
 import os
 
 import numpy as np
 import pytest
 
 import binary_oracle as bo
-from particles_b200 import _lib, binary_smc as bs, distributions as dists
-from test_smc2_host import _c_struct_fields
+from particles_b200 import binary_smc as bs, distributions as dists
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 G = np.load(os.path.join(HERE, "golden", "golden_binary.npz"))
 DESIGNS = {"p10": bo.small_design, "p104": bo.boston_like}
-
-
-def test_vs_desc_layout_matches_header():
-    with open(os.path.join(HERE, "..", "include", "smcb.h")) as f:
-        src = f.read()
-    fields = _c_struct_fields(src, "smcb_vs_desc")
-    assert [n for n, _ in fields] == [n for n, _ in _lib.VsDesc._fields_]
-    size = {"int32_t": 4, "double": 8, "ptr": 8}
-    off = 0
-    for (nm, ct), (pn, pt) in zip(fields, _lib.VsDesc._fields_):
-        s = size[ct]
-        off = (off + s - 1) // s * s
-        assert getattr(_lib.VsDesc, pn).offset == off, nm
-        assert C.sizeof(pt) == s, nm
-        off += s
-    assert C.sizeof(_lib.VsDesc) == off
 
 
 @pytest.mark.parametrize("tag", ["p10", "p104"])

@@ -1,7 +1,6 @@
-"""CPU-side tests: the C-ABI library loads and exports every symbol include/smcb.h
-declares, the host logic that maps Feynman-Kac objects onto fused kernels, the Philox
-restatement used by the GPU tests, and the no-CPU-fallback rule.  No compute calls."""
-import ctypes
+"""CPU-side tests: the library is built for sm_90a only, the host logic that maps
+Feynman-Kac objects onto fused kernels, the Philox restatement used by the GPU tests, and
+the no-CPU-fallback rule.  No compute calls."""
 import os
 import re
 import subprocess
@@ -15,58 +14,11 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import philox_ref  # noqa: E402
 
 
-@pytest.fixture(scope="module")
-def lib():
-    from particles_b200 import _lib, build
-    build.build()
-    return _lib.load()
-
-
-def header_symbols():
-    txt = open(os.path.join(ROOT, "include", "smcb.h")).read()
-    txt = re.sub(r"/\*.*?\*/", "", txt, flags=re.S)
-    return sorted(set(re.findall(r"\b(smcb_[a-z0-9_]+)\s*\(", txt)))
-
-
-def test_library_exports_every_declared_symbol(lib):
-    from particles_b200 import _lib
-    syms = header_symbols()
-    assert len(syms) >= 25
-    raw = ctypes.CDLL(_lib.SO_PATH)
-    for s in syms:
-        assert hasattr(raw, s), f"{s} declared in include/smcb.h but not exported"
-    assert set(_lib.PROTOTYPES) == set(syms)          # the ctypes layer binds exactly the header
-    assert lib.smcb_version() == 100
-    assert lib.smcb_resample_scratch_doubles(1000, 500) >= 1000 + 500
-
-
 def test_built_for_sm_90a_only():
     from particles_b200 import _lib
     out = subprocess.run(["cuobjdump", "-lelf", _lib.SO_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
     assert archs == {"90a"}, archs
-
-
-def test_filter_desc_layout_matches_header():
-    """ctypes mirror of smcb_filter_desc: every field at the same offset as in the C struct."""
-    from particles_b200 import _lib
-    D = _lib.FilterDesc
-    names = [f[0] for f in D._fields_]
-    probes = ", ".join(f"offsetof(smcb_filter_desc, {n})" for n in names)
-    fmt = " ".join(["%zu"] * (len(names) + 1))
-    src = f'''
-    #include <stdio.h>
-    #include <stddef.h>
-    #include "smcb.h"
-    int main(void) {{ printf("{fmt}\\n", sizeof(smcb_filter_desc), {probes}); return 0; }}
-    '''
-    exe = os.path.join(ROOT, "oracle", "_build", "layout_probe")
-    os.makedirs(os.path.dirname(exe), exist_ok=True)
-    subprocess.run(["gcc", "-x", "c", "-", "-I", os.path.join(ROOT, "include"), "-o", exe],
-                   input=src, text=True, check=True)
-    vals = [int(v) for v in subprocess.run([exe], capture_output=True, text=True).stdout.split()]
-    assert vals[0] == ctypes.sizeof(D)
-    assert dict(zip(names, vals[1:])) == {n: getattr(D, n).offset for n in names}
 
 
 def test_philox_known_answers():

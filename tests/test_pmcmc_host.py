@@ -1,38 +1,16 @@
-"""Particle MCMC pieces that need no device: the conditional-filter descriptor against include/smcb.h, the
-combinations the samplers refuse, PMMH's host logic against the live reference's chain (tests/golden/golden_pmcmc.npz),
-the oracle CSMC against the reference's history and trajectories, the host build of the pinned weight against the
-oracle's logG, and the Gibbs update order."""
+"""Particle MCMC pieces that need no device: the combinations the samplers refuse, PMMH's host logic against the live
+reference's chain (tests/golden/golden_pmcmc.npz), the oracle CSMC against the reference's history and trajectories,
+the host build of the pinned weight against the oracle's logG, and the Gibbs update order."""
 import ctypes as C
 import os
-import re
 
 import numpy as np
 import pytest
 from oracle import pmcmc_numpy as pmo
 from oracle.smc_numpy import LinearGauss as OLG
 from particles_b200 import _lib, bank, distributions as dists, kalman, mcmc, state_space_models as ssm
-from test_smc2_host import _c_struct_fields
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def test_csmc_desc_layout_matches_header():
-    with open(os.path.join(HERE, "..", "include", "smcb.h")) as f:
-        src = f.read()
-    fields = _c_struct_fields(src, "smcb_csmc_desc")
-    assert [n for n, _ in fields] == [n for n, _ in _lib.CsmcDesc._fields_]
-    size = {"int32_t": 4, "int64_t": 8, "double": 8, "ptr": 8, "uint64_t": 8}
-    off = 0
-    for (nm, ct), (pn, pt) in zip(fields, _lib.CsmcDesc._fields_):
-        s = size[ct]
-        off = (off + s - 1) // s * s
-        assert getattr(_lib.CsmcDesc, pn).offset == off, nm
-        assert C.sizeof(pt) == s, nm
-        off += s
-    assert C.sizeof(_lib.CsmcDesc) == off
-    assert int(re.search(r"#define SMCB_CSMC_BACKWARD (\d+)", src).group(1)) == _lib.CSMC_BACKWARD
-    for name in ("smcb_csmc_plan", "smcb_csmc_run"):
-        assert name in _lib.PROTOTYPES and re.search(r"\bint " + name + r"\(", src)
 
 
 PRIOR = dists.StructDist({"rho": dists.Uniform(a=-1.0, b=1.0)})

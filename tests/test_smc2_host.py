@@ -1,17 +1,11 @@
 """SMC^2 pieces that need no device: the theta -> model-constant map against the scalar specs, the static-parameter
-laws against scipy, the filter-bank descriptor against include/smcb.h, and the sampler's host logic (exchange
-trigger, Nx bookkeeping, waste-free reshape) over a stub bank."""
-import ctypes as C
-import os
-import re
-
+laws against scipy, and the sampler's host logic (exchange trigger, Nx bookkeeping, waste-free reshape) over a stub
+bank."""
 import numpy as np
 import pytest
 from scipy import stats
 
-from particles_b200 import _lib, bank, kalman, state_space_models as ssm
-
-HERE = os.path.dirname(os.path.abspath(__file__))
+from particles_b200 import bank, kalman, state_space_models as ssm
 
 MODELS = {
     "StochVol": (ssm.StochVol, ssm.spec_stochvol, {"mu": (-2, 0), "rho": (0.5, 0.99), "sigma": (0.05, 1)}),
@@ -92,42 +86,6 @@ def test_static_laws_vs_scipy():
     ref = (stats.uniform.logpdf(th["phi"], loc=-1, scale=2) + stats.beta.logpdf(th["rho"], 9.0, 1.0)
            + stats.gamma.logpdf(th["sigma"], 2.0, scale=0.5))
     np.testing.assert_allclose(prior.logpdf(th), ref, rtol=1e-12)
-
-
-def _c_struct_fields(src, name):
-    body = re.search(r"typedef struct \{([^{}]*)\}\s*" + name + ";", src).group(1)
-    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
-    fields = []
-    for decl in body.split(";"):
-        decl = decl.strip()
-        if not decl:
-            continue
-        m = re.match(r"(const\s+)?([\w]+)\s*(\*?)\s*(.*)", decl)
-        ctype, star, names = m.group(2), m.group(3), m.group(4)
-        for nm in names.split(","):
-            nm = nm.strip().lstrip("*")
-            fields.append((nm, "ptr" if star or "*" in names else ctype))
-    return fields
-
-
-def test_bank_desc_layout_matches_header():
-    with open(os.path.join(HERE, "..", "include", "smcb.h")) as f:
-        src = f.read()
-    fields = _c_struct_fields(src, "smcb_bank_desc")
-    assert [n for n, _ in fields] == [n for n, _ in _lib.BankDesc._fields_]
-    size = {"int32_t": 4, "int64_t": 8, "double": 8, "ptr": 8, "uint64_t": 8}
-    off = 0
-    for (nm, ct), (pn, pt) in zip(fields, _lib.BankDesc._fields_):
-        s = size[ct]
-        off = (off + s - 1) // s * s
-        assert getattr(_lib.BankDesc, pn).offset == off, nm
-        assert C.sizeof(pt) == s, nm
-        off += s
-    assert C.sizeof(_lib.BankDesc) == off
-    assert int(re.search(r"#define SMCB_BANK_STATE (\d+)", src).group(1)) == _lib.BANK_STATE
-    for name in ("smcb_bank_plan", "smcb_bank_advance", "smcb_bank_gather", "smcb_bank_merge", "smcb_bank_keys",
-                 "smcb_mh_accept_flags"):
-        assert name in _lib.PROTOTYPES and re.search(r"\bint " + name + r"\(", src)
 
 
 # ---------------------------------------------------------------------------------------------- host logic, stub bank

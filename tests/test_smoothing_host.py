@@ -178,29 +178,6 @@ def test_transition_spec_recogniser():
     assert np.array_equal(g["step_consts"], [8.0 * np.cos(1.2 * (t - 1)) for t in range(5)])
 
 
-def test_smooth_desc_layout_matches_header():
-    """ctypes mirror of smcb_smooth_desc: every field at the same offset as in the C struct."""
-    import subprocess
-    from particles_b200 import _lib
-    D = _lib.SmoothDesc
-    names = [f[0] for f in D._fields_]
-    probes = ", ".join(f"offsetof(smcb_smooth_desc, {n})" for n in names)
-    fmt = " ".join(["%zu"] * (len(names) + 1))
-    src = f'''
-    #include <stdio.h>
-    #include <stddef.h>
-    #include "smcb.h"
-    int main(void) {{ printf("{fmt}\\n", sizeof(smcb_smooth_desc), {probes}); return 0; }}
-    '''
-    exe = os.path.join(ROOT, "oracle", "_build", "smooth_layout_probe")
-    os.makedirs(os.path.dirname(exe), exist_ok=True)
-    subprocess.run(["gcc", "-x", "c", "-", "-I", os.path.join(ROOT, "include"), "-o", exe], input=src, text=True,
-                   check=True)
-    vals = [int(v) for v in subprocess.run([exe], capture_output=True, text=True).stdout.split()]
-    assert vals[0] == C.sizeof(D)
-    assert dict(zip(names, vals[1:])) == {n: getattr(D, n).offset for n in names}
-
-
 def test_bound_methods_follow_the_reference():
     from particles_b200 import state_space_models as ssm
     fk = ssm.Bootstrap(ssm=ssm.StochVol(), data=[np.zeros(1)] * 3)

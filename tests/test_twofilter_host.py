@@ -1,7 +1,6 @@
 """Two-filter smoothing on the CPU: the NumPy oracle (tests/twofilter_oracle.py) against the live reference's
-estimates (tests/golden/golden_twofilter.npz, written by make_golden_twofilter.py), the ctypes mirror of
-smcb_twofilter_desc against the header, and smoothing_worker's method table."""
-import ctypes as C
+estimates (tests/golden/golden_twofilter.npz, written by make_golden_twofilter.py), and smoothing_worker's
+method table."""
 import os
 import sys
 
@@ -93,31 +92,6 @@ def test_golden_draws_fit_their_histories(gt):
             for k in ("I", "J"):
                 a = gt[f"{name}/{tag}_{k}"]
                 assert a.dtype == np.int16 and a.min() >= 0 and a.max() < n
-
-
-def test_twofilter_desc_layout_matches_header():
-    """ctypes mirror of smcb_twofilter_desc: every field at the same offset as in the C struct."""
-    import subprocess
-    from particles_b200 import _lib
-    D = _lib.TwoFilterDesc
-    names = [f[0] for f in D._fields_]
-    probes = ", ".join(f"offsetof(smcb_twofilter_desc, {n})" for n in names)
-    fmt = " ".join(["%zu"] * (len(names) + 1))
-    src = f'''
-    #include <stdio.h>
-    #include <stddef.h>
-    #include "smcb.h"
-    int main(void) {{ printf("{fmt}\\n", sizeof(smcb_twofilter_desc), {probes}); return 0; }}
-    '''
-    exe = os.path.join(ROOT, "oracle", "_build", "twofilter_layout_probe")
-    os.makedirs(os.path.dirname(exe), exist_ok=True)
-    subprocess.run(["gcc", "-x", "c", "-", "-I", os.path.join(ROOT, "include"), "-o", exe], input=src, text=True,
-                   check=True)
-    vals = [int(v) for v in subprocess.run([exe], capture_output=True, text=True).stdout.split()]
-    assert vals[0] == C.sizeof(D)
-    assert dict(zip(names, vals[1:])) == {n: getattr(D, n).offset for n in names}
-    assert (_lib.TF_ON2_ROWS, _lib.TF_ON_LOGW) == (0, 1)
-    assert "smcb_two_filter" in _lib.PROTOTYPES
 
 
 def test_smoothing_worker_method_table():
