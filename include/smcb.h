@@ -138,6 +138,43 @@ int smcb_mvnormal_logpdf(smcb_ctx *ctx, const double *x, const double *loc,
 int smcb_standard_normal(smcb_ctx *ctx, double *out, int64_t n);
 int smcb_uniform(smcb_ctx *ctx, double *out, int64_t n);
 
+/* The laws of distributions.py with a kernel of their own (csrc/smcb_dists.cuh), by law code:
+ *   0 InvGamma(a, b)                  :358-377  scipy.stats.invgamma.logpdf(x, a, scale=b); draws b / Gamma(a, 1)
+ *   1 LogNormal(mu, sigma)            :379-396  scipy.stats.lognorm.logpdf(x, sigma, scale=exp(mu))
+ *   2 TruncNormal(mu, sigma, a, b)    :475-505  scipy.stats.truncnorm.logpdf, mass in log space; exact draws
+ *   3 Binomial(n, p)                  :535-549  scipy.stats.binom.logpmf
+ *   4 Geometric(p)                    :552-565  scipy.stats.geom.logpmf (support 1, 2, ...)
+ *   5 NegativeBinomial(n, p)          :568-595  scipy.stats.nbinom.logpmf(x, n, p), the law its draws follow
+ *   6 DiscreteUniform(lo, hi)         :631-649  -log(hi - lo) on lo .. hi - 1
+ *   7 Gamma(a, rate b)                draws only: the sampler InvGamma, NegativeBinomial and Dirichlet draw through
+ * Parameter k is the array pk of n values, or NULL and the scalar s[k] (s: host array of 4 doubles; unused ones
+ * are ignored).  NaN outside a law's parameter domain, -inf outside its support and, for codes 3-6, at non-integer
+ * x.  Draws: fp64 into out for codes 0-2 and 7, int64 for the discrete codes 3-6 (INT64_MIN where a parameter is
+ * outside its domain); element i's draw depends on (seed, API call, i) only. */
+int smcb_dist_logpdf(smcb_ctx *ctx, int law, const double *x, double x0, const double *p0, const double *p1,
+                     const double *p2, const double *p3, const double *s, double *out, int64_t n);
+int smcb_dist_rvs(smcb_ctx *ctx, int law, const double *p0, const double *p1, const double *p2, const double *p3,
+                  const double *s, void *out, int64_t n);
+/* Dirichlet(alpha), distributions.py:854-885: alpha (d,) on the device, rows x (n, d) with row stride x_ld (0: one
+ * row for all n); c0 = -log B(alpha).  *bad (device int, zeroed by the caller) collects the bits of the tests of
+ * scipy.stats.dirichlet's input check that some row fails (the host raises its ValueError): 1 an entry < 0 or > 1,
+ * 2 a zero entry where alpha_j < 1, 4 |sum - 1| > 1e-9, 8 a NaN entry (which, as in scipy, voids test 1 and makes
+ * the row's density NaN).  rvs: Gamma(alpha_j, 1) draws normalised in log space (finite for small alphas). */
+int smcb_dirichlet_logpdf(smcb_ctx *ctx, const double *x, int64_t x_ld, const double *alpha, int d, double c0,
+                          double *out, int *bad, int64_t n);
+int smcb_dirichlet_rvs(smcb_ctx *ctx, const double *alpha, int d, double *out, int64_t n);
+/* VaryingCovNormal, distributions.py:1012-1059, 1 <= d <= 8 (SMCB_ENOSYS above): cov, L (n, d, d) row-major; chol
+ * writes the lower factors and sets *bad (device int, zeroed by the caller) when a cov[i] is not positive
+ * definite; loc / x rows of d values with row stride loc_ld / x_ld (0: one row for all n). */
+int smcb_vcn_chol(smcb_ctx *ctx, const double *cov, int d, double *L, int *bad, int64_t n);
+int smcb_vcn_rvs(smcb_ctx *ctx, const double *loc, int64_t loc_ld, const double *L, int d, double *out, int64_t n);
+int smcb_vcn_logpdf(smcb_ctx *ctx, const double *x, int64_t x_ld, const double *loc, int64_t loc_ld,
+                    const double *L, int d, double *out, int64_t n);
+/* Mixture.logpdf, distributions.py:805-810: out[i] = logsumexp_j (logpk[i pk_ld + j] + lp[j n + i]), lp the (k, n)
+ * component log-densities, logpk (k,) (pk_ld = 0) or (n, k) (pk_ld = k) */
+int smcb_mixture_logpdf(smcb_ctx *ctx, const double *lp, const double *logpk, int64_t pk_ld, int k, double *out,
+                        int64_t n);
+
 /* ---------------------------------------------------------------------------
  * SMC samplers: tempering / waste-free move step  (particles/smc_samplers.py)
  * theta is (n, d) row-major, d <= 32

@@ -20,6 +20,11 @@ FK_BOOTSTRAP, FK_GUIDED, FK_APF, FK_AUXBOOT = 0, 1, 2, 3
 MODEL_STOCHVOL, MODEL_LINGAUSS, MODEL_GORDON, MODEL_THETALOGISTIC = 0, 1, 2, 3
 MODEL_BEARINGS, MODEL_MVLINGAUSS, MODEL_DISCRETECOX, MODEL_STOCHVOLLEV = 4, 5, 6, 7
 LSE_SUM, LSE_MEAN, LSE_ESSL = 0, 1, 2
+# law codes of smcb_dist_logpdf / smcb_dist_rvs
+LAW_INVGAMMA, LAW_LOGNORMAL, LAW_TRUNCNORMAL, LAW_BINOMIAL, LAW_GEOMETRIC = 0, 1, 2, 3, 4
+LAW_NEGBINOMIAL, LAW_DISCRETEUNIFORM, LAW_GAMMA = 5, 6, 7
+# bits of smcb_dirichlet_logpdf's *bad: the tests of scipy.stats.dirichlet's input check
+DIRICHLET_RANGE, DIRICHLET_ZERO, DIRICHLET_SUM, DIRICHLET_NAN = 1, 2, 4, 8
 
 c_dp = C.c_void_p  # device pointers travel as integers
 
@@ -224,6 +229,16 @@ PROTOTYPES = {
                                        C.c_int64]),
     "smcb_standard_normal": (C.c_int, [C.c_void_p, c_dp, C.c_int64]),
     "smcb_uniform": (C.c_int, [C.c_void_p, c_dp, C.c_int64]),
+    "smcb_dist_logpdf": (C.c_int, [C.c_void_p, C.c_int, c_dp, C.c_double, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp,
+                                   C.c_int64]),
+    "smcb_dist_rvs": (C.c_int, [C.c_void_p, C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, C.c_int64]),
+    "smcb_dirichlet_logpdf": (C.c_int, [C.c_void_p, c_dp, C.c_int64, c_dp, C.c_int, C.c_double, c_dp, c_dp,
+                                        C.c_int64]),
+    "smcb_dirichlet_rvs": (C.c_int, [C.c_void_p, c_dp, C.c_int, c_dp, C.c_int64]),
+    "smcb_vcn_chol": (C.c_int, [C.c_void_p, c_dp, C.c_int, c_dp, c_dp, C.c_int64]),
+    "smcb_vcn_rvs": (C.c_int, [C.c_void_p, c_dp, C.c_int64, c_dp, C.c_int, c_dp, C.c_int64]),
+    "smcb_vcn_logpdf": (C.c_int, [C.c_void_p, c_dp, C.c_int64, c_dp, C.c_int64, c_dp, C.c_int, c_dp, C.c_int64]),
+    "smcb_mixture_logpdf": (C.c_int, [C.c_void_p, c_dp, c_dp, C.c_int64, C.c_int, c_dp, C.c_int64]),
     "smcb_logistic_target": (C.c_int, [C.c_void_p, c_dp, C.c_int64, C.c_int, c_dp, C.c_int64, C.c_double,
                                        C.c_double, c_dp, c_dp, c_dp]),
     "smcb_logistic_wf_move": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, c_dp, c_dp, c_dp, c_dp, c_dp,

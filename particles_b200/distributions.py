@@ -94,6 +94,15 @@ class Normal(LocScaleDist):
                                               ptr(out), n))
         return out
 
+    def posterior(self, x, sigma=1.0):
+        """particles/distributions.py:279-285: X_1..X_n ~ N(theta, sigma^2), theta ~ self (host arithmetic)."""
+        x = _host(x)
+        pr0 = 1.0 / _host(self.scale) ** 2
+        prd = x.size / sigma ** 2
+        varp = 1.0 / (pr0 + prd)
+        mu = varp * (pr0 * _host(self.loc) + prd * x.mean())
+        return Normal(loc=mu, scale=np.sqrt(varp))
+
 
 class _Univariate(ProbDist):
     """logpdf through the elementwise kernel smcb_logpdf1 (kinds: 0 Student, 1 Gamma, 2 Laplace, 3 Logistic)."""
@@ -151,6 +160,11 @@ class Gamma(_Univariate):
     def logpdf(self, x):
         from scipy.special import gammaln
         return self._call(x, float(self.a), -gammaln(float(self.a)), self.b, 1.0)
+
+    def posterior(self, x):
+        """particles/distributions.py:353-355: X_1..X_n ~ N(0, 1/theta), theta ~ self."""
+        x = _host(x)
+        return Gamma(a=self.a + 0.5 * x.size, b=self.b + 0.5 * np.sum(x ** 2))
 
     def rvs(self, size=None):
         b = as_device(self.b) if isinstance(self.b, (torch.Tensor, np.ndarray)) else \
@@ -272,9 +286,13 @@ class StructDist(ProbDist):
         return out
 
 
-class Categorical(ProbDist):
-    """Categorical(p), p (k,) or (N, k) -- particles/distributions.py:598-628."""
+class DiscreteDist(ProbDist):
+    """Base class of the discrete laws -- particles/distributions.py:513-516: ``rvs`` returns int64 CUDA tensors."""
     dtype = np.int64
+
+
+class Categorical(DiscreteDist):
+    """Categorical(p), p (k,) or (N, k) -- particles/distributions.py:598-628."""
 
     def __init__(self, p=None):
         if p is None:
@@ -322,10 +340,9 @@ class MixMissing(ProbDist):
         return x
 
 
-class Poisson(ProbDist):
+class Poisson(DiscreteDist):
     """Poisson(rate) -- particles/distributions.py:519-532 (logpdf on the device; ``rate`` a CUDA
     tensor or scalar, ``x`` the observed count).  scipy evaluates xlogy(k, mu) - gammaln(k+1) - mu."""
-    dtype = np.int64
 
     def __init__(self, rate=1.0):
         self.rate = rate
@@ -480,3 +497,449 @@ class MvNormal(ProbDist):
         _lib.check(ctx.lib.smcb_mvnormal_logpdf(ctx.handle, ptr(xs), ptr(la), self._hp(l0), ptr(sa),
                                                 self._hp(s0), self._hp(L), d, ptr(out), n))
         return out
+
+    def posterior(self, x, Sigma=None):
+        """particles/distributions.py:984-1009: X_1..X_n ~ N(theta, Sigma), theta ~ self; scale must be one."""
+        import scipy.linalg as sla
+        if np.any(_host(self.scale) != 1.0):
+            raise ValueError("posterior of MvNormal: scale must be one.")
+        x = _host(x)
+        n = x.shape[0]
+        Sigma = np.eye(self.dim) if Sigma is None else _host(Sigma)
+        Siginv = sla.inv(Sigma)
+        covinv = sla.inv(self.cov)
+        Sigpost = sla.inv(covinv + n * Siginv)
+        loc = _host(self.loc)
+        m = np.full(self.dim, float(loc)) if loc.ndim == 0 else loc
+        mupost = Sigpost @ (m @ covinv + Siginv @ np.sum(x, axis=0))
+        return MvNormal(loc=mupost, cov=Sigpost)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# laws of the elementwise kernels smcb_dist_logpdf / smcb_dist_rvs (csrc/smcb_dists.cuh)
+# ---------------------------------------------------------------------------------------------------------------------
+def _common_length(size, *arrs):
+    lens = {int(a.shape[0]) for a in arrs if a is not None}
+    if len(lens) > 1:
+        raise ValueError(f"operands could not be broadcast together with lengths {sorted(lens)}")
+    if lens:
+        return lens.pop()
+    return 1 if size is None else int(size)
+
+
+class _KernelLaw(ProbDist):
+    """A law with a device log-density and sampler (law code ``_law`` of include/smcb.h).  Its parameters,
+    ``_params()``, are scalars or (N,) arrays / tensors: array parameters make it a Markov kernel, as for Normal."""
+    _law = None
+
+    def _params(self):
+        raise NotImplementedError
+
+    def _args(self):
+        ps = [_split(v) for v in self._params()]
+        arrays = [a for a, _ in ps] + [None] * (4 - len(ps))
+        scalars = np.array([v for _, v in ps] + [0.0] * (4 - len(ps)), dtype=np.float64)
+        return arrays, scalars
+
+    def logpdf(self, x):
+        xa, x0 = _split(x)
+        arrays, scalars = self._args()
+        n = _common_length(None, xa, *arrays)
+        ctx = context()
+        out = empty(n)
+        _lib.check(ctx.lib.smcb_dist_logpdf(ctx.handle, self._law, ptr(xa), x0, *[ptr(a) for a in arrays],
+                                            scalars.ctypes.data_as(C.c_void_p), ptr(out), n))
+        return out
+
+    def rvs(self, size=None):
+        arrays, scalars = self._args()
+        n = _common_length(size, *arrays)
+        if size is not None and int(size) != n:        # numpy.random's broadcast error
+            raise ValueError(f"shape mismatch: {n} parameter values cannot be broadcast to size {int(size)}")
+        ctx = context()
+        out = empty(n, dtype=torch.int64 if self.dtype == np.int64 else torch.float64)
+        _lib.check(ctx.lib.smcb_dist_rvs(ctx.handle, self._law, *[ptr(a) for a in arrays],
+                                         scalars.ctypes.data_as(C.c_void_p), ptr(out), n))
+        return out
+
+
+class InvGamma(_KernelLaw):
+    """Inverse Gamma(a, b) -- particles/distributions.py:358-377 (scipy.stats.invgamma(a, scale=b)); draws
+    b / Gamma(a, 1) from the device Gamma sampler."""
+    _law = _lib.LAW_INVGAMMA
+
+    def __init__(self, a=1.0, b=1.0):
+        self.a, self.b = a, b
+
+    def _params(self):
+        return self.a, self.b
+
+    def posterior(self, x):
+        """particles/distributions.py:374-376: X_1..X_n ~ N(0, theta), theta ~ self."""
+        x = _host(x)
+        return InvGamma(a=self.a + 0.5 * x.size, b=self.b + 0.5 * np.sum(x ** 2))
+
+
+class LogNormal(_KernelLaw):
+    """Law of exp(X), X ~ N(mu, sigma^2) -- particles/distributions.py:379-396."""
+    _law = _lib.LAW_LOGNORMAL
+
+    def __init__(self, mu=0.0, sigma=1.0):
+        self.mu, self.sigma = mu, sigma
+
+    def _params(self):
+        return self.mu, self.sigma
+
+
+class TruncNormal(_KernelLaw):
+    """N(mu, sigma^2) truncated to [a, b] -- particles/distributions.py:475-505.  The log mass is computed in log
+    space (finite in either far tail) and the draws are exact (smcb_dists.cuh: truncnorm_std_rvs)."""
+    _law = _lib.LAW_TRUNCNORMAL
+
+    def __init__(self, mu=0.0, sigma=1.0, a=0.0, b=1.0):
+        self.mu, self.sigma, self.a, self.b = mu, sigma, a, b
+        self.au = (a - mu) / sigma
+        self.bu = (b - mu) / sigma
+
+    def _params(self):
+        return self.mu, self.sigma, self.a, self.b
+
+    def posterior(self, x, s=1.0):
+        """particles/distributions.py:499-505: X_1..X_n ~ N(theta, s^2), theta ~ self."""
+        x = _host(x)
+        pr0 = 1.0 / _host(self.sigma) ** 2
+        prd = x.size / s ** 2
+        varp = 1.0 / (pr0 + prd)
+        mu = varp * (pr0 * _host(self.mu) + prd * x.mean())
+        return TruncNormal(mu=mu, sigma=np.sqrt(varp), a=self.a, b=self.b)
+
+
+class FlatNormal(ProbDist):
+    """Normal with infinite variance, the law of a missing value -- particles/distributions.py:435-451: log-density
+    zero of the broadcast shape of x and loc, draws loc + NaN."""
+
+    def __init__(self, loc=0.0):
+        self.loc = loc
+
+    def logpdf(self, x):
+        return torch.zeros(np.broadcast_shapes(np.shape(x), np.shape(self.loc)), dtype=torch.float64, device="cuda")
+
+    def rvs(self, size=None):
+        sz = 1 if size is None else int(size)
+        loc = as_device(self.loc) if isinstance(self.loc, (torch.Tensor, np.ndarray)) else float(self.loc)
+        return loc + torch.full((sz,), float("nan"), dtype=torch.float64, device="cuda")
+
+
+class Binomial(DiscreteDist, _KernelLaw):
+    """Binomial(n, p) -- particles/distributions.py:535-549.  logpdf is scipy.stats.binom.logpmf (Loader's
+    saddle-point form: accurate for large n); draws by inversion while n min(p, 1 - p) < 10, BTRS otherwise."""
+    _law = _lib.LAW_BINOMIAL
+
+    def __init__(self, n=1, p=0.5):
+        self.n, self.p = n, p
+
+    def _params(self):
+        return self.n, self.p
+
+
+class Geometric(DiscreteDist, _KernelLaw):
+    """Geometric(p) on 1, 2, ... -- particles/distributions.py:552-565."""
+    _law = _lib.LAW_GEOMETRIC
+
+    def __init__(self, p=0.5):
+        self.p = p
+
+    def _params(self):
+        return (self.p,)
+
+
+class NegativeBinomial(DiscreteDist, _KernelLaw):
+    """Number of failures before the n-th success, p the success probability -- particles/distributions.py:568-595.
+    Draws as numpy.random.negative_binomial(n, p): Poisson(Gamma(n, scale (1 - p) / p)).  logpdf is
+    scipy.stats.nbinom.logpmf(x, n, p), the law of those draws; the reference's line 592 passes (p, n) in swapped
+    order (DESIGN.md section 5.16)."""
+    _law = _lib.LAW_NEGBINOMIAL
+
+    def __init__(self, n=1, p=0.5):
+        self.n, self.p = n, p
+
+    def _params(self):
+        return self.n, self.p
+
+
+class DiscreteUniform(DiscreteDist, _KernelLaw):
+    """Uniform on lo, lo + 1, ..., hi - 1 -- particles/distributions.py:631-649."""
+    _law = _lib.LAW_DISCRETEUNIFORM
+
+    def __init__(self, lo=0, hi=2):
+        self.lo, self.hi = lo, hi
+        width = hi - lo
+        self.log_norm_cst = width.double().log() if isinstance(width, torch.Tensor) else np.log(width)
+
+    def _params(self):
+        return self.lo, self.hi
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# transforms, mixtures, conditional laws: host composition over the device laws
+# ---------------------------------------------------------------------------------------------------------------------
+def _mod(x):
+    """torch for tensors, NumPy for everything else."""
+    return torch if isinstance(x, torch.Tensor) else np
+
+
+class TransformedDist(ProbDist):
+    """Law of Y = f(X), X ~ base_dist -- particles/distributions.py:657-697.  ``f``, ``finv`` and ``logJac`` take
+    CUDA tensors (state-space models) and NumPy arrays (a field of a StructDist's structured array) alike."""
+
+    def __init__(self, base_dist):
+        self.base_dist = base_dist
+
+    def error_msg(self, method):
+        return f'method {method} not defined in class {self.__class__}'
+
+    def f(self, x):
+        raise NotImplementedError(self.error_msg("f"))
+
+    def finv(self, x):
+        """Inverse of f."""
+        raise NotImplementedError(self.error_msg("finv"))
+
+    def logJac(self, x):
+        """Log of the Jacobian of finv."""
+        raise NotImplementedError(self.error_msg("logJac"))
+
+    def rvs(self, size=None):
+        return self.f(self.base_dist.rvs(size=size))
+
+    def logpdf(self, x):
+        lp = self.base_dist.logpdf(self.finv(x))
+        if isinstance(x, torch.Tensor):
+            lp = as_device(lp)
+        else:
+            lp = _host(lp)
+        return lp + self.logJac(x)
+
+
+class LinearD(TransformedDist):
+    """Y = a X + b -- particles/distributions.py:700-724."""
+
+    def __init__(self, base_dist, a=1.0, b=0.0):
+        self.a, self.b = a, b
+        self.base_dist = base_dist
+
+    def f(self, x):
+        return self.a * x + self.b
+
+    def finv(self, x):
+        return (x - self.b) / self.a
+
+    def logJac(self, x):
+        return -np.log(self.a)
+
+
+class LogD(TransformedDist):
+    """Y = log(X) -- particles/distributions.py:727-746."""
+
+    def f(self, x):
+        return _mod(x).log(x)
+
+    def finv(self, x):
+        return _mod(x).exp(x)
+
+    def logJac(self, x):
+        return x
+
+
+class LogitD(TransformedDist):
+    """Y = logit((X - a) / (b - a)) -- particles/distributions.py:749-775.  logJac's log(1 + exp(x)) is a softplus,
+    max(x, 0) + log1p(exp(-|x|)), finite where the reference's overflows (x > ~709; DESIGN.md section 5.16)."""
+
+    def __init__(self, base_dist, a=0.0, b=1.0):
+        self.a, self.b = a, b
+        self.base_dist = base_dist
+
+    def f(self, x):
+        p = (x - self.a) / (self.b - self.a)
+        return _mod(x).log(p / (1.0 - p))
+
+    def finv(self, x):
+        return self.a + (self.b - self.a) / (1.0 + _mod(x).exp(-x))
+
+    def logJac(self, x):
+        m = _mod(x)
+        softplus = m.maximum(x, 0.0 * x) + m.log1p(m.exp(-m.abs(x)))
+        return np.log(self.b - self.a) + x - 2.0 * softplus
+
+
+class Mixture(ProbDist):
+    """Mixture of k laws -- particles/distributions.py:783-816; pk (k,) or (N, k).  logpdf: the components' device
+    log-densities, then one row log-sum-exp kernel; rvs: a categorical index per element from the context's
+    Philox stream, then the chosen component's draw."""
+
+    def __init__(self, pk, *components):
+        self.pk = pk if isinstance(pk, torch.Tensor) else np.atleast_1d(pk)
+        self.k = self.pk.shape[-1]
+        if len(components) != self.k:
+            raise ValueError("Size of pk and nr of components should match")
+        self.components = components
+
+    def _pk(self):
+        """pk on the device; a (1, k) pk is the (k,) one"""
+        pk = as_device(self.pk)
+        return pk.reshape(-1) if pk.ndim == 2 and pk.shape[0] == 1 else pk
+
+    def _length(self, pk, cols):
+        """common length of the (n,) columns and the rows of a 2-D pk; length 1 broadcasts, as in NumPy"""
+        lens = {int(v.shape[0]) for v in cols} | ({int(pk.shape[0])} if pk.ndim == 2 else set())
+        if len(lens - {1}) > 1:
+            raise ValueError(f"Mixture: operands could not be broadcast together with lengths {sorted(lens)}")
+        return max(lens)
+
+    def logpdf(self, x):
+        lps = [as_device(cd.logpdf(x)).reshape(-1) for cd in self.components]
+        pk = self._pk()
+        n = self._length(pk, lps)
+        lp = torch.stack([v.expand(n) for v in lps]).contiguous()
+        logpk = torch.log(pk).contiguous()
+        ctx = context()
+        out = empty(n)
+        _lib.check(ctx.lib.smcb_mixture_logpdf(ctx.handle, ptr(lp), ptr(logpk), self.k if pk.ndim == 2 else 0,
+                                               self.k, ptr(out), n))
+        return out
+
+    def rvs(self, size=None):
+        pk = self._pk()
+        xk = [as_device(cd.rvs(size=size)).reshape(-1) for cd in self.components]
+        n = self._length(pk, xk)
+        u = Uniform().rvs(size=n)
+        idx = (torch.cumsum(pk, -1) < u[:, None]).sum(-1).clamp_(max=self.k - 1)     # searchsorted(cumsum(pk), u)
+        return torch.stack([v.expand(n) for v in xk]).gather(0, idx.reshape(1, -1)).reshape(-1)
+
+
+class Cond(ProbDist):
+    """Conditional law in a StructDist -- particles/distributions.py:1130-1146: ``law`` maps the structured array
+    drawn so far to a law."""
+
+    def __init__(self, law, dim=1, dtype="float64"):
+        self.law = law
+        self.dim = dim
+        self.dtype = dtype
+
+    def __call__(self, x):
+        return self.law(x)
+
+
+class Dirichlet(ProbDist):
+    """Dirichlet(alphas), alphas (d,) -- particles/distributions.py:854-885.  logpdf of rows x (N, d) (or one (d,)
+    point) on the device, with scipy.stats.dirichlet's ValueError for points off the simplex (its tests and
+    tolerance, |sum - 1| <= 1e-9); rvs (size, d) from device Gamma draws normalised in log space."""
+
+    def __init__(self, alphas=None):
+        if alphas is None:
+            raise ValueError('Dirichlet: missing parameter alphas')
+        self.alphas = alphas
+
+    @property
+    def dim(self):
+        return self.alphas.shape[0]
+
+    def _alpha(self):
+        a = _host(self.alphas)
+        if a.ndim != 1 or np.any(~(a > 0)):
+            raise ValueError("All parameters must be greater than 0")
+        return a
+
+    def logpdf(self, x):
+        from scipy.special import gammaln
+        a = self._alpha()
+        d = a.shape[0]
+        xd = as_device(x)
+        xd = xd.reshape(1, -1) if xd.ndim == 1 else xd
+        if xd.shape[-1] == d - 1:                          # scipy appends the last coordinate
+            xd = torch.cat([xd, 1.0 - xd.sum(-1, keepdim=True)], dim=-1)
+        if xd.ndim != 2 or xd.shape[-1] != d:
+            raise ValueError(f"Vector 'x' must have either the same number of entries as, or one entry fewer than, "
+                             f"parameter vector 'a', but alpha.shape = {a.shape} and x.shape = {tuple(xd.shape)}.")
+        xd = xd.contiguous()
+        n = xd.shape[0]
+        ctx = context()
+        out = empty(n)
+        bad = torch.zeros(1, dtype=torch.int32, device=out.device)
+        _lib.check(ctx.lib.smcb_dirichlet_logpdf(ctx.handle, ptr(xd), d, ptr(as_device(a)), d,
+                                                 float(gammaln(a.sum()) - gammaln(a).sum()), ptr(out), ptr(bad), n))
+        flags = int(bad.item())
+        if flags & _lib.DIRICHLET_RANGE and not flags & _lib.DIRICHLET_NAN:
+            raise ValueError("Each entry in 'x' must be greater than or equal to zero, and smaller or equal one.")
+        if flags & _lib.DIRICHLET_ZERO:
+            raise ValueError("Each entry in 'x' must be greater than zero if its alpha is less than one.")
+        if flags & _lib.DIRICHLET_SUM:
+            raise ValueError("The input vector 'x' must lie within the normal simplex.")
+        return out
+
+    def rvs(self, size=1):
+        a = self._alpha()
+        n = 1 if size is None else int(size)
+        ctx = context()
+        out = empty((n, a.shape[0]))
+        _lib.check(ctx.lib.smcb_dirichlet_rvs(ctx.handle, ptr(as_device(a)), a.shape[0], ptr(out), n))
+        return out
+
+
+class VaryingCovNormal(MvNormal):
+    """Multivariate normal with one covariance matrix per particle -- particles/distributions.py:1012-1059.
+    ``cov`` (N, d, d), d <= 8; the constructor computes the N Cholesky factors on the device (``.L``, an (N, d, d)
+    tensor) and raises ValueError when a cov[n] is not positive definite.  ``loc``: scalar, (d,) or (N, d)."""
+
+    def __init__(self, loc=0.0, cov=None):
+        self.loc = loc
+        err_msg = "VaryingCovNormal: argument cov must be a (N, d, d) array, \
+                with d>1; cov[n, :, :] must be symmetric and positive"
+        if cov is None or len(np.shape(cov)) != 3 or np.shape(cov)[1] != np.shape(cov)[2]:
+            raise ValueError(err_msg)
+        self.cov = as_device(cov)
+        self.N, d, _ = self.cov.shape
+        if d > 8:
+            raise NotImplementedError(f"VaryingCovNormal: d = {d}; the device kernels take d <= 8")
+        ctx = context()
+        self.L = empty((self.N, d, d))
+        bad = torch.zeros(1, dtype=torch.int32, device=self.L.device)
+        _lib.check(ctx.lib.smcb_vcn_chol(ctx.handle, ptr(self.cov), d, ptr(self.L), ptr(bad), self.N))
+        if int(bad.item()):
+            raise ValueError(err_msg)
+
+    def _rows(self, v, what):
+        """-> (device rows, row stride): a scalar, a (d,) vector or a (1, d) row is one row for every particle (stride
+        0), an (N, d) array one row per particle; any other shape is NumPy's broadcast ValueError."""
+        d = self.dim
+        v = as_device(v)
+        if v.ndim == 0 or (v.ndim == 1 and v.shape[0] == 1):
+            return v.reshape(1).expand(d).contiguous(), 0
+        if v.ndim == 1 and v.shape[0] == d:
+            return v, 0
+        if v.ndim == 2 and v.shape[1] == d and v.shape[0] in (1, self.N):
+            return v.contiguous(), (0 if v.shape[0] == 1 else d)
+        raise ValueError(f"VaryingCovNormal: {what} of shape {tuple(v.shape)} does not broadcast against the "
+                         f"({self.N}, {d}) particles")
+
+    def rvs(self, size=None):
+        N = self.N if size is None else int(size)
+        if N != self.N:
+            raise ValueError(f"VaryingCovNormal.rvs: size {N} for {self.N} covariance matrices")
+        loc, loc_ld = self._rows(self.loc, "loc")
+        ctx = context()
+        out = empty((N, self.dim))
+        _lib.check(ctx.lib.smcb_vcn_rvs(ctx.handle, ptr(loc), loc_ld, ptr(self.L), self.dim, ptr(out), N))
+        return out
+
+    def logpdf(self, x):
+        xr, x_ld = self._rows(x, "x")
+        loc, loc_ld = self._rows(self.loc, "loc")
+        ctx = context()
+        out = empty(self.N)
+        _lib.check(ctx.lib.smcb_vcn_logpdf(ctx.handle, ptr(xr), x_ld, ptr(loc), loc_ld, ptr(self.L), self.dim,
+                                           ptr(out), self.N))
+        return out
+
+    def posterior(self, x, Sigma=None):
+        raise NotImplementedError
