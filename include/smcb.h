@@ -396,6 +396,34 @@ int smcb_filter_state(smcb_filter *f, double *out8);
 int smcb_filter_fusion_stats(smcb_filter *f, int64_t *out3);
 
 /* ---------------------------------------------------------------------------
+ * sequential quasi-Monte Carlo  (particles/core.py:315-349, rqmc.py, hilbert.py)
+ * ------------------------------------------------------------------------- */
+/* rqmc.sobol(n, d) for 1 <= d <= 32: scipy.stats.qmc.Sobol's 30-bit points 0 .. n-1, squeezed into
+ * u = 0.5 + (1 - 1e-10) (p - 0.5); u and raw (the 30-bit integers) are component-major (d, n), either may be NULL.
+ * scramble != 0: a random lower-triangular bit matrix and digital shift per dimension, drawn from Philox under
+ * (seed, call); scramble = 0: scipy's scramble=False points, bit for bit. */
+int smcb_sobol(smcb_ctx *ctx, int d, int64_t n, int scramble, uint64_t seed, uint64_t call, double *u,
+               int32_t *raw);
+/* hilbert.hilbert_sort(x) for SoA (d, n) points, 1 <= d <= 32: order = np.argsort(x) for d = 1, otherwise the
+ * argsort of the int64 Hilbert keys of floor(invlogit(standardised x) * floor(2^(62/d))), which wrap as the
+ * reference's do (signed comparison).  keys (d > 1, may be NULL) = the unsorted keys.  Equal keys come out in any
+ * order.  scratch: smcb_hilbert_scratch_bytes(n, d) bytes, 256-byte aligned (-1: bad sizes). */
+int64_t smcb_hilbert_scratch_bytes(int64_t n, int d);
+int smcb_hilbert_sort(smcb_ctx *ctx, const double *x, int64_t n, int d, int64_t *order, int64_t *keys,
+                      void *scratch);
+/* nsteps SQMC steps (resample_move_qmc, always resampling) of a filter made by smcb_filter_create, which fixes the
+ * model, kind, buffers and seed (desc.scheme and desc.essrmin are ignored; desc.moments must be NULL).  Step t draws
+ * the points of smcb_sobol(du (+ 1), n, 1, desc.seed, t) with du = the state dimension -- or, when desc.u_in is not
+ * NULL, the caller's points: T blocks of (du + 1, n) doubles, component-major, step 0 reading the first du rows of
+ * block 0 (parity tests against recorded point sets) -- writes X[t & 1], lw[t & 1],
+ * A and summary row t (rs_flag 1 from t = 1).  No host sync.  scratch: smcb_sqmc_scratch_bytes(n, dim) bytes,
+ * 256-byte aligned (-1: bad sizes). */
+int64_t smcb_sqmc_scratch_bytes(int64_t n, int dim);
+/* out = Phi^-1(u) (scipy.special.ndtri, within 8 ulp on the squeezed Sobol' range): the ppf of Normal and MvNormal */
+int smcb_ndtri(smcb_ctx *ctx, const double *u, double *out, int64_t n);
+int smcb_sqmc_step(smcb_filter *f, int64_t nsteps, void *scratch);
+
+/* ---------------------------------------------------------------------------
  * off-line smoothing: FFBS backward sampling over a stored history (particles/smoothing.py:278-423)
  * ------------------------------------------------------------------------- */
 #define SMCB_SMOOTH_ON2 0    /* backward_sampling_ON2,    smoothing.py:291-311 */

@@ -279,6 +279,12 @@ PROTOTYPES = {
     "smcb_filter_step_timed": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_double)]),
     "smcb_filter_state": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),
     "smcb_filter_fusion_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
+    "smcb_sobol": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_uint64, C.c_uint64, c_dp, c_dp]),
+    "smcb_hilbert_scratch_bytes": (C.c_int64, [C.c_int64, C.c_int]),
+    "smcb_hilbert_sort": (C.c_int, [C.c_void_p, c_dp, C.c_int64, C.c_int, c_dp, c_dp, c_dp]),
+    "smcb_sqmc_scratch_bytes": (C.c_int64, [C.c_int64, C.c_int]),
+    "smcb_sqmc_step": (C.c_int, [C.c_void_p, C.c_int64, c_dp]),
+    "smcb_ndtri": (C.c_int, [C.c_void_p, c_dp, c_dp, C.c_int64]),
     "smcb_backward_sample": (C.c_int, [C.c_void_p, C.POINTER(SmoothDesc)]),
     "smcb_online_smooth": (C.c_int, [C.c_void_p, C.POINTER(OnlineDesc)]),
     "smcb_two_filter": (C.c_int, [C.c_void_p, C.POINTER(TwoFilterDesc)]),

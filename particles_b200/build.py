@@ -17,7 +17,7 @@ SO = os.path.join(HERE, "libsmcb.so")
 SOURCES = ["smcb_api.cu", "smcb_filter.cu", "smcb_filter_1d.cu", "smcb_filter_nd.cu", "smcb_sampler.cu",
            "smcb_smooth.cu", "smcb_online.cu", "smcb_variance.cu", "smcb_batch.cu", "smcb_bank.cu", "smcb_pmcmc.cu",
            "smcb_nested.cu", "smcb_binary.cu", "smcb_twofilter.cu", "smcb_hmm.cu",
-           "smcb_kalman.cu", "smcb_dists.cu"]
+           "smcb_kalman.cu", "smcb_dists.cu", "smcb_sqmc.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)
 NVCC_FLAGS = GENCODE + [
     "-O3", "-lineinfo", "-std=c++17",

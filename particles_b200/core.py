@@ -234,6 +234,53 @@ class _FusedEngine:
             pass
 
 
+class _SqmcEngine(_FusedEngine):
+    """A fused filter stepped by SQMC (csrc/smcb_sqmc.cu): the buffers, summary table and attributes of
+    ``_FusedEngine``; every step resamples through the Hilbert order of the particles (core.py:339-349).
+    ``points``: None (Sobol' points of key (seed, t)) or, per step t, the (N, du + 1) points to use ((N, du) at t = 0),
+    as the reference's ``rqmc.sobol`` would return them."""
+
+    def __init__(self, spec, N, seed, points=None):
+        u_in = None
+        if points is not None:
+            dim = int(spec.get("dim", 1))
+            T = int(spec["data"].shape[0])
+            if len(points) < T:
+                raise ValueError(f"SQMC points: need one point set per step ({T}), got {len(points)}")
+            u_in = np.zeros((T, dim + 1, N))
+            for t in range(T):
+                p = np.asarray(points[t], dtype=np.float64).reshape(N, -1)
+                rows = dim if t == 0 else dim + 1
+                if p.shape[1] < rows:
+                    raise ValueError(f"SQMC points of step {t}: need {rows} columns, got {p.shape[1]}")
+                u_in[t, :rows] = p[:, :rows].T
+        super().__init__(spec, N, "systematic", 0.5, seed, noise=None if u_in is None else (None, u_in))
+        nb = int(self.lib.smcb_sqmc_scratch_bytes(self.N, self.dim))
+        if nb < 0:
+            raise ValueError(f"SQMC: bad sizes (N={self.N}, dim={self.dim})")
+        self._scratch = torch.empty(nb + 256, dtype=torch.uint8, device=self.ctx.device)
+        base = self._scratch.data_ptr()
+        self._scratch_ptr = base + (-base) % 256
+        self._t = 0
+
+    def step(self, nsteps=1):
+        self.ctx.bind_stream()
+        _lib.check(self.lib.smcb_sqmc_step(self.handle, int(nsteps), self._scratch_ptr))
+        self._t += int(nsteps)
+
+    def step_timed(self, nsteps):
+        raise NotImplementedError("step_timed runs the SMC step kernel; time SQMC with CUDA events around step()")
+
+    def fusion_stats(self):
+        raise NotImplementedError("an SQMC filter fuses no streaming steps")
+
+    def weight_stats(self):
+        lw = self.lw[(self._t - 1) & 1].clone()
+        st = torch.empty(4, dtype=torch.float64, device=lw.device)
+        _lib.check(self.lib.smcb_normalise(self.ctx.handle, ptr(lw), self.N, None, ptr(st)))
+        return st
+
+
 class _P2PPool:
     """Peer-mapped memory of one (process, process group): ONE mailbox and one (growing) arena per rank, allocated
     and exchanged once -- a single tensor all-gather of the 64-byte CUDA IPC handles -- and then reused by every
@@ -378,8 +425,6 @@ class SMC:
         _lib.load()
         from .smc_samplers import from_reference_smc2
         fk = from_reference_smc2(fk) or fk          # the reference's SMC2 of a stock 1-D model: the filter bank
-        if qmc:
-            raise NotImplementedError("SQMC (qmc=True) is outside the accelerated path")
         if resampling not in rs.rs_funcs:
             raise ValueError(f"{resampling} is not a valid resampling scheme")
         self.fk, self.N, self.qmc = fk, N, qmc
@@ -401,7 +446,15 @@ class SMC:
                 spec = None                      # residual, ssp, killing, ...: plugin path (stand-alone kernels)
             if spec is None and fused is True:
                 raise NotImplementedError("this Feynman-Kac model has no fused kernel")
-        if spec is not None:
+            if qmc:
+                spec = fused_spec(fk)            # SQMC ignores the resampling scheme, as the reference does
+        if qmc:
+            self._qmc_points = None if noise is None else [np.asarray(p.cpu() if torch.is_tensor(p) else p,
+                                                                      dtype=np.float64) for p in noise]
+        if spec is not None and qmc:
+            self._engine = _SqmcEngine(spec, N, self._seed, self._qmc_points)
+            self._row_cache = {}
+        elif spec is not None:
             # collect=[Moments()] with the default mom_func: the step kernel accumulates sum w x / sum w x^2 next
             # to its log-sum-exp triple and writes a (T, 8) table -- run() keeps its sync-free fast path
             self._dev_moments = self.summaries is not None and self.summaries.device_moments(fk)
@@ -453,6 +506,16 @@ class SMC:
     @X.setter
     def X(self, v):
         self._p["X"] = v
+
+    @property
+    def h_order(self):
+        """SQMC: the Hilbert order of the particles the last step resampled from (core.py:344)."""
+        if not self.qmc or self._done < 2:
+            raise AttributeError("h_order exists after a resampling step of SQMC (qmc=True)")
+        if not self.fused:
+            return self._p["h_order"]
+        from .hilbert import hilbert_order
+        return hilbert_order(self._engine.X[self._done & 1])     # generation t - 1 (step s writes X[s & 1])
 
     @property
     def rs_flag(self):
@@ -528,7 +591,36 @@ class SMC:
         return out
 
     def generate_particles(self):                             # core.py:315-321
-        self._p["X"] = self.fk.M0(self.N)
+        if self.qmc:
+            u = self._points(self.fk.du)
+            self._p["X"] = self.fk.Gamma0(u[:, 0].contiguous() if u.shape[1] == 1 else u)
+        else:
+            self._p["X"] = self.fk.M0(self.N)
+
+    def _points(self, d):
+        """(N, d) points of step t on the plugin path: the injected ones, or the Sobol' points of key (seed, t) that
+        the fused SQMC engine draws."""
+        if self._qmc_points is not None:
+            return as_device(np.ascontiguousarray(self._qmc_points[self.t].reshape(self.N, -1)[:, :d]))
+        from .rqmc import sobol_points
+        return sobol_points(self.N, d, self._seed, self.t).t().contiguous()
+
+    def resample_move_qmc(self):                              # core.py:339-349
+        from .hilbert import hilbert_order, hilbert_sort
+        p = self._p
+        p["rs_flag"] = True
+        du = self.fk.du
+        u = self._points(du + 1)
+        tau = hilbert_order(u[:, 0].contiguous())            # argsort of one coordinate
+        h = hilbert_sort(p["X"])
+        p["h_order"] = h
+        su = self._gather(u[:, 0].contiguous(), tau)
+        idx = rs.inverse_cdf(su, self._gather(p["aux"].W, h))
+        p["A"] = self._gather(h.view(torch.float64), idx).view(torch.int64)     # h[idx]: an 8-byte copy
+        p["Xp"] = self._gather(p["X"], p["A"])
+        v = self._gather(u[:, 1:].contiguous(), tau)
+        self.reset_weights()
+        p["X"] = self.fk.Gamma(self.t, p["Xp"], v[:, 0].contiguous() if du == 1 else v)
 
     def reweight_particles(self):                             # core.py:323-324
         p = self._p
@@ -583,7 +675,10 @@ class SMC:
             self.generate_particles()
         else:
             self.setup_auxiliary_weights()
-            self.resample_move()
+            if self.qmc:
+                self.resample_move_qmc()
+            else:
+                self.resample_move()
         self.reweight_particles()
         self.compute_summaries()
         self.t += 1

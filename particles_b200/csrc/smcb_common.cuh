@@ -109,6 +109,7 @@ enum : uint32_t {
     kPurposeTraj = 6,         // the uniform of the conditional SMC trajectory draw at step t
     kPurposeHmm = 7,          // the uniform of trajectory n's draw at step t of HMM b
     kPurposeDists = 8,        // block b of element n's draw in the samplers of smcb_dists.cuh (API call in word 2)
+    kPurposeSobol = 9,        // word block b of the Sobol' scrambling of dimension j (smcb_sqmc.cuh; call in word 2)
 };
 constexpr uint64_t kOnlineSeedMix = 0x9E3779B97F4A7C15ull;   // the on-line smoothers' key: seed ^ kOnlineSeedMix
 

@@ -149,6 +149,12 @@ __device__ __forceinline__ void mtab_issue(const double *gsrc, uint64_t *bar) {
     mbar_arrive_expect_tx(bar, (uint32_t)kMathTabBytes);
     tma_bulk_g2s(const_cast<double *>(mtab()), gsrc, (uint32_t)kMathTabBytes, bar);
 }
+// stage the tables of a CTA whose dynamic shared memory starts with them: issue, then everybody waits
+__device__ __forceinline__ void stage_math_tables(const double *gsrc, uint64_t *bar) {
+    if (threadIdx.x == 0) mtab_issue(gsrc, bar);
+    __syncthreads();
+    mbar_wait(bar, 0);
+}
 #endif
 
 constexpr double kExpScaleT = (double)kExpTabN * SMCB_LOG2E;

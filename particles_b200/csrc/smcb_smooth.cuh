@@ -85,10 +85,7 @@ __device__ __forceinline__ void warp_lse_merge(double &mx, double &s) {
 
 template <class M>
 __device__ __forceinline__ void stage_tables(const double *tab, uint64_t *bar, bool needed) {
-    if (!needed) return;
-    if (threadIdx.x == 0) mtab_issue(tab, bar);
-    __syncthreads();
-    mbar_wait(bar, 0);
+    if (needed) stage_math_tables(tab, bar);
 }
 
 // the exact draw of smoothing.py:418-421 for ONE target xs, by the whole warp:

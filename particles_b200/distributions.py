@@ -19,6 +19,15 @@ from .device import as_device, context, empty, ptr
 HALFLOG2PI = 0.5 * np.log(2.0 * np.pi)
 
 
+def ndtri(u):
+    """Phi^-1(u) on the device (csrc/smcb_sqmc.cuh; within 8 ulp of scipy.special.ndtri on the squeezed range)."""
+    u = as_device(u)
+    out = torch.empty_like(u)
+    ctx = context()
+    _lib.check(ctx.lib.smcb_ndtri(ctx.handle, ptr(u), ptr(out), u.numel()))
+    return out
+
+
 def _split(v):
     """scalar-or-array argument -> (device tensor or None, scalar).  A size-1 array or tensor is a scalar that
     broadcasts -- ``StateSpaceModel.simulate`` returns observations of shape (1,), and NumPy broadcasts
@@ -82,6 +91,10 @@ class Normal(LocScaleDist):
         out = empty(n)
         _lib.check(ctx.lib.smcb_normal_rvs(ctx.handle, ptr(la), l0, ptr(sa), s0, ptr(zd), ptr(out), n))
         return out
+
+    def ppf(self, u):
+        """scipy.stats.norm.ppf(u, loc, scale) = loc + scale * Phi^-1(u), on the device."""
+        return self.rvs(z=ndtri(u))
 
     def logpdf(self, x):
         xa, x0 = _split(x)
@@ -373,6 +386,9 @@ class Dirac(ProbDist):
         n = 1 if size is None else size
         return torch.full((n,), float(self.loc), dtype=torch.float64, device="cuda")
 
+    def ppf(self, u):
+        return self.rvs(size=u.shape[0])                 # distributions.py:471-472
+
     def logpdf(self, x):
         x = as_device(x)
         loc = self.loc if isinstance(self.loc, torch.Tensor) else float(self.loc)
@@ -405,6 +421,11 @@ class IndepProd(ProbDist):
                 cols.append(d.rvs(size=size, z=as_device(z)[:, k].contiguous()))
                 k += 1
         return torch.stack(cols, dim=1)
+
+    def ppf(self, u):
+        """Column i of u through law i's ppf (distributions.py:1108-1109)."""
+        u = as_device(u)
+        return torch.stack([d.ppf(u[..., i].contiguous()) for i, d in enumerate(self.dists)], dim=1)
 
 
 class IID(IndepProd):
@@ -480,6 +501,16 @@ class MvNormal(ProbDist):
         _lib.check(ctx.lib.smcb_mvnormal_rvs(ctx.handle, ptr(la), self._hp(l0), ptr(sa), self._hp(s0),
                                              self._hp(L), d, ptr(zd), ptr(out), n))
         return out.t().contiguous()
+
+    def ppf(self, u):
+        """Rosenblatt transform through the Cholesky factor, loc + scale * Phi^-1(u) @ L.T; when u has fewer than d
+        columns the remaining ones of z are 0 (distributions.py:971-983)."""
+        u = as_device(u)
+        u = u.reshape(u.shape[0], -1)
+        z = ndtri(u)
+        if z.shape[1] < self.dim:
+            z = torch.cat([z, torch.zeros((z.shape[0], self.dim - z.shape[1]), dtype=z.dtype, device=z.device)], 1)
+        return self.rvs(z=z)
 
     def logpdf(self, x):
         d = self.dim

@@ -159,8 +159,7 @@ class ParticleHistory(RollingParticleHistory):
         return self._backward(_lib.SMOOTH_REJECT, M, seed, noise, max_trials=max_trials, bounds=bounds)
 
     def backward_sampling_qmc(self, M):
-        raise NotImplementedError("QMC backward sampling needs SQMC (qmc=True), which is outside the "
-                                  "accelerated path")
+        raise NotImplementedError("QMC backward sampling (of an SQMC history) is not built")
 
     # ------------------------------------------------------------ two-filter
     def two_filter_smoothing(self, t, info, phi, loggamma, linear_cost=False, return_ess=False,
@@ -473,14 +472,15 @@ def smoothing_worker(method=None, N=100, fk=None, fk_info=None, add_func=None, l
     Returns {"est": (T-1,) array, "cpu": seconds}: the estimates stay on the device until one read at the end, and
     ``cpu`` is the wall time of the runs plus the smoothing, ending with that read.  'FFBS_purereject' is the
     hybrid sampler with 2^24 - 1 proposals per draw before the exact draw (the reference allows N * 10^9);
-    'FFBS_QMC' raises NotImplementedError (SQMC is not built); an unknown method raises ValueError."""
+    'FFBS_QMC' raises NotImplementedError (QMC backward sampling of an SQMC history is not built); an unknown method raises ValueError."""
     import time
 
     from .core import SMC
     if method not in WORKER_METHODS:
         raise ValueError(f"smoothing_worker: no such method {method!r}; one of {WORKER_METHODS}")
     if method == "FFBS_QMC":
-        raise NotImplementedError("smoothing_worker: FFBS_QMC needs SQMC, which is not built")
+        raise NotImplementedError("smoothing_worker: FFBS_QMC needs QMC backward sampling of an SQMC history, "
+                                  "which is not built")
     T = fk.T
     if fk_info is None:
         fk_info = fk.__class__(ssm=fk.ssm, data=fk.data[::-1])

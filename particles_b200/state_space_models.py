@@ -91,6 +91,17 @@ class Bootstrap(FeynmanKac):
     def M(self, t, xp):
         return self.ssm.PX(t, xp).rvs(size=xp.shape[0])
 
+    @property
+    def du(self):
+        """Dimension of the uniforms of SQMC (state_space_models.py:320)."""
+        return self.ssm.PX0().dim
+
+    def Gamma0(self, u):
+        return self.ssm.PX0().ppf(u)
+
+    def Gamma(self, t, xp, u):
+        return self.ssm.PX(t, xp).ppf(u)
+
     def logG(self, t, xp, x):
         return self.ssm.PY(t, xp, x).logpdf(self.data[t])
 
@@ -114,6 +125,12 @@ class GuidedPF(Bootstrap):
 
     def M(self, t, xp):
         return self.ssm.proposal(t, xp, self.data).rvs(size=xp.shape[0])
+
+    def Gamma0(self, u):
+        return self.ssm.proposal0(self.data).ppf(u)
+
+    def Gamma(self, t, xp, u):
+        return self.ssm.proposal(t, xp, self.data).ppf(u)
 
     def logG(self, t, xp, x):
         if t == 0:
