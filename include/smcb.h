@@ -398,10 +398,11 @@ int smcb_filter_fusion_stats(smcb_filter *f, int64_t *out3);
 /* ---------------------------------------------------------------------------
  * sequential quasi-Monte Carlo  (particles/core.py:315-349, rqmc.py, hilbert.py)
  * ------------------------------------------------------------------------- */
-/* rqmc.sobol(n, d) for 1 <= d <= 32: scipy.stats.qmc.Sobol's 30-bit points 0 .. n-1, squeezed into
+/* rqmc.sobol(n, d) for 1 <= d <= 4096: scipy.stats.qmc.Sobol's 30-bit points 0 .. n-1, squeezed into
  * u = 0.5 + (1 - 1e-10) (p - 0.5); u and raw (the 30-bit integers) are component-major (d, n), either may be NULL.
  * scramble != 0: a random lower-triangular bit matrix and digital shift per dimension, drawn from Philox under
- * (seed, call); scramble = 0: scipy's scramble=False points, bit for bit. */
+ * (seed, call, dimension), so that dimension j's points do not depend on d; scramble = 0: scipy's scramble=False
+ * points, bit for bit. */
 int smcb_sobol(smcb_ctx *ctx, int d, int64_t n, int scramble, uint64_t seed, uint64_t call, double *u,
                int32_t *raw);
 /* hilbert.hilbert_sort(x) for SoA (d, n) points, 1 <= d <= 32: order = np.argsort(x) for d = 1, otherwise the
@@ -458,6 +459,10 @@ typedef struct {
     int64_t *idx;              /* out (T, M): idx[T-1] = idx_T; GATHER: input                       */
     double *paths;             /* out (T, M, dim) = X[t][idx[t]]                                    */
     int64_t *counts;           /* reject: out (T-1, 2) {accepted, proposals} (zeroed here)          */
+    /* ON2 only: NULL (index order), or a device array of T-1 device pointers, order[t] a permutation of 0 .. N-1:
+       the draw at t walks the CDF of particles order[t][0], order[t][1], ... (QMC backward sampling over the
+       Hilbert orders of an SQMC history, smoothing.py:425-455); idx stays in particle indices */
+    const int64_t *const *order;
 } smcb_smooth_desc;
 
 /* ONE kernel launch for the whole backward pass (plus a memset of counts for reject); no host sync */

@@ -60,7 +60,7 @@ class SmoothDesc(C.Structure):
         ("X", c_dp), ("lw", c_dp), ("A", c_dp), ("x_stride_n", C.c_int64), ("x_stride_c", C.c_int64),
         ("log_bound", c_dp), ("cdf", c_dp), ("cdf_ld", C.c_int64), ("idx_T", c_dp),
         ("u", c_dp), ("prop", c_dp), ("lu", c_dp), ("u_exact", c_dp),
-        ("idx", c_dp), ("paths", c_dp), ("counts", c_dp),
+        ("idx", c_dp), ("paths", c_dp), ("counts", c_dp), ("order", c_dp),
     ]
 
 

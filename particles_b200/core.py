@@ -509,11 +509,14 @@ class SMC:
 
     @property
     def h_order(self):
-        """SQMC: the Hilbert order of the particles the last step resampled from (core.py:344)."""
+        """SQMC: the Hilbert order of the particles the last step resampled from (core.py:344).  On the plugin path it
+        exists from inside step 1 on, as in the reference, so that ``hist.save`` records it for t = 1."""
+        if not self.fused:
+            if not self.qmc or self._p.get("h_order") is None:
+                raise AttributeError("h_order exists after a resampling step of SQMC (qmc=True)")
+            return self._p["h_order"]
         if not self.qmc or self._done < 2:
             raise AttributeError("h_order exists after a resampling step of SQMC (qmc=True)")
-        if not self.fused:
-            return self._p["h_order"]
         from .hilbert import hilbert_order
         return hilbert_order(self._engine.X[self._done & 1])     # generation t - 1 (step s writes X[s & 1])
 

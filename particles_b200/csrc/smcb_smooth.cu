@@ -3,7 +3,8 @@
 // launch that loops over t = T-2 ... 0 inside, with no grid-wide synchronisation:
 //   ON2     one CTA owns 256 trajectories; per t it walks tiles of (loc(X_t[n]), lw_t[n]) staged in shared memory
 //           (the transition location computed ONCE per particle and shared by the CTA's trajectories), pass 1 an
-//           online (max, sum exp) per trajectory, pass 2 the re-walk to the crossing of u * S with early exit;
+//           online (max, sum exp) per trajectory, pass 2 the re-walk to the crossing of u * S with early exit; with
+//           a per-t order table (QMC backward sampling) both passes walk the particles in that order;
 //   MCMC    one thread per trajectory: chain started at the genealogy, nsteps independent Metropolis steps with
 //           multinomial proposals from W_t (inverse CDF on the caller's per-t CDF);
 //   REJECT  one thread per trajectory, lanes in lockstep over t: at most max_trials proposals, then a
@@ -35,7 +36,9 @@ __device__ __forceinline__ StepK step_at(const smcb_smooth_desc &d, int64_t t) {
 // ---------------------------------------------------------------------------
 // ON2 -- smoothing.py:291-311
 // ---------------------------------------------------------------------------
-template <class M>
+// ORD: tile position p holds particle d.order[t][p], so the CDF accumulates in that order and the crossing found maps
+// back through it (smoothing.py:445-452); !ORD: position p holds particle p
+template <class M, bool ORD>
 __global__ void __launch_bounds__(kSmBlock) k_bs_on2(M m, smcb_smooth_desc d, Philox key, uint64_t call,
                                                     const double *tab) {
     constexpr int D = M::D;
@@ -59,8 +62,9 @@ __global__ void __launch_bounds__(kSmBlock) k_bs_on2(M m, smcb_smooth_desc d, Ph
         const double *lw = d.lw[t];
         auto fill = [&](int64_t base) {
             __syncthreads();                               // the previous tile is consumed
-            const int64_t n = base + threadIdx.x;
-            if (n < N) {
+            const int64_t pos = base + threadIdx.x;
+            if (pos < N) {
+                const int64_t n = ORD ? d.order[t][pos] : pos;
                 double xp[D], lc[D];
                 load_x<D>(d, t, n, xp);
                 td.loc(m, k, xp, lc);
@@ -109,7 +113,7 @@ __global__ void __launch_bounds__(kSmBlock) k_bs_on2(M m, smcb_smooth_desc d, Ph
         }
         if (live) {
             if (found < 0) found = last >= 0 ? last : 0;       // round-off / all-zero row (smcb_smooth.cuh)
-            nxt = found;
+            nxt = ORD ? d.order[t][found] : found;
             load_x<D>(d, t, nxt, xn);
             put_path<D>(d, t, j, nxt, xn);
         }
@@ -292,8 +296,12 @@ int run_model(smcb_ctx *c, const smcb_smooth_desc &d) {
     const size_t tab = TransUsesTable<M>::value ? kMathTabBytes : 0;
     if (d.method == SMCB_SMOOTH_ON2) {
         const size_t smem = kMathTabBytes + (size_t)(M::D + 1) * kSmBlock * sizeof(double);
-        SMCB_TRY(set_smem(k_bs_on2<M>, smem));
-        return launch(c, k_bs_on2<M>, grid, kSmBlock, smem, m, d, key, call, c->math_tab);
+        if (d.order) {
+            SMCB_TRY(set_smem(k_bs_on2<M, true>, smem));
+            return launch(c, k_bs_on2<M, true>, grid, kSmBlock, smem, m, d, key, call, c->math_tab);
+        }
+        SMCB_TRY(set_smem(k_bs_on2<M, false>, smem));
+        return launch(c, k_bs_on2<M, false>, grid, kSmBlock, smem, m, d, key, call, c->math_tab);
     }
     if (d.method == SMCB_SMOOTH_MCMC) {
         SMCB_TRY(set_smem(k_bs_mcmc<M>, tab));
@@ -317,6 +325,7 @@ extern "C" int smcb_backward_sample(smcb_ctx *c, const smcb_smooth_desc *dp) {
     SMCB_REQUIRE(d.method >= SMCB_SMOOTH_ON2 && d.method <= SMCB_SMOOTH_REJECT, "smcb_backward_sample: bad method %d",
                  (int)d.method);
     SMCB_REQUIRE(d.lw && d.idx_T, "smcb_backward_sample: NULL log-weights or final indices");
+    SMCB_REQUIRE(!d.order || d.method == SMCB_SMOOTH_ON2, "smcb_backward_sample: an order table needs ON2");
     if (d.method == SMCB_SMOOTH_MCMC) {
         SMCB_REQUIRE(d.nsteps >= 0 && d.nsteps < (1 << 24), "smcb_backward_sample: nsteps out of range");
         SMCB_REQUIRE(d.T == 1 || d.A, "smcb_backward_sample: MCMC needs the ancestors");

@@ -21,33 +21,38 @@ constexpr int kThreads = 256;
 constexpr int kColBlocks = 128;   // most CTAs per column of the Hilbert standardisation (col_stats)
 
 // ------------------------------------------------------------------------------------------------------------- Sobol
-// every CTA builds the scrambled direction numbers of the d dimensions in shared memory, then writes its points
+constexpr int kSobolSlab = 32;    // dimensions per CTA row of the grid (blockIdx.y)
+
+// every CTA builds the scrambled direction numbers of its slab of up to kSobolSlab dimensions in shared memory, then
+// writes their points; dimension j's numbers are keyed by j alone, so its points do not depend on d or on the slab
 __global__ void k_sobol(int d, int64_t n, int scramble, Philox key, uint64_t call, double *u, int32_t *raw) {
-    __shared__ uint32_t words[kSobolMaxDim][32];
-    __shared__ uint32_t sv[kSobolMaxDim][kSobolBits];
-    __shared__ uint32_t shift[kSobolMaxDim];
+    __shared__ uint32_t words[kSobolSlab][32];
+    __shared__ uint32_t sv[kSobolSlab][kSobolBits];
+    __shared__ uint32_t shift[kSobolSlab];
     auto gen = [&](uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t r[4]) {
         philox4x32_10(c0, c1, c2, c3, key.k0, key.k1, r);
     };
-    for (int j = threadIdx.x; j < d; j += blockDim.x) {
-        sobol_scramble_words(gen, j, call, words[j]);
+    const int j0 = blockIdx.y * kSobolSlab, dj = min(kSobolSlab, d - j0);
+    for (int j = threadIdx.x; j < dj; j += blockDim.x) {
+        sobol_scramble_words(gen, j0 + j, call, words[j]);
         uint32_t v[kSobolBits], s;
-        sobol_dims(j, scramble, words[j], v, s);
+        sobol_dims(j0 + j, scramble, words[j], v, s);
         for (int k = 0; k < kSobolBits; k++) sv[j][k] = v[k];
         shift[j] = s;
     }
     __syncthreads();
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        for (int j = 0; j < d; j++) {
+        for (int j = 0; j < dj; j++) {
             const uint32_t q = sobol_int(sv[j], shift[j], (uint64_t)i);
-            if (raw) raw[j * n + i] = (int32_t)q;
-            if (u) u[j * n + i] = squeeze(q);
+            if (raw) raw[(j0 + j) * n + i] = (int32_t)q;
+            if (u) u[(j0 + j) * n + i] = squeeze(q);
         }
     }
 }
 
 int sobol(smcb_ctx *c, int d, int64_t n, int scramble, uint64_t seed, uint64_t call, double *u, int32_t *raw) {
-    return launch(c, k_sobol, grid_for(n, kThreads), kThreads, 0, d, n, scramble, key_of(seed), call, u, raw);
+    const dim3 grid(grid_for(n, kThreads), (d + kSobolSlab - 1) / kSobolSlab);
+    return launch(c, k_sobol, grid, kThreads, 0, d, n, scramble, key_of(seed), call, u, raw);
 }
 
 // ----------------------------------------------------------------------------------------------------------- Hilbert

@@ -7,8 +7,10 @@
 #ifndef SMCB_SQMC_HOST_TEST
 #include "smcb_common.cuh"
 #define SMCB_SOBOL_CONST __constant__ const
+#define SMCB_SOBOL_GLOBAL __device__ const
 #else
 #define SMCB_SOBOL_CONST static const
+#define SMCB_SOBOL_GLOBAL static const
 #endif
 
 namespace smcb {
@@ -17,6 +19,7 @@ namespace sqmc {
 #define SMCB_HD __host__ __device__ __forceinline__
 
 #include "smcb_sobol_dirs.inc"
+#include "smcb_sobol_init.inc"
 
 #ifdef SMCB_SQMC_HOST_TEST
 constexpr uint32_t kPurposeSobol = 9;     // as in smcb_common.cuh
@@ -133,11 +136,34 @@ SMCB_HD void sobol_scramble_words(const KEY &key_fn, int j, uint64_t call, uint3
     }
 }
 
+// the direction numbers of dimension j, 1 <= j < kSobolMaxDim, from its primitive polynomial p of degree s and its s
+// initial numbers (smcb_sobol_init.inc), by scipy's recurrence (_initialize_v):
+//   m_k = m_{k-s} ^ (2^s m_{k-s}) ^ XOR_{i < s-1, bit s-1-i of p} 2^(i+1) m_{k-i-1},
+// then number k = m_k 2^(29-k).  For j < kSobolTabDim this reproduces kSobolDirs (tests/test_ffbs_qmc_host.py).
+SMCB_HD void sobol_expand(int j, uint32_t v[kSobolBits]) {
+    const uint32_t *row = kSobolInit + kSobolInitOff[j];
+    const uint32_t p = row[0];
+    int s = 0;
+    while ((p >> (s + 1)) != 0u) s++;
+    for (int k = 0; k < s; k++) v[k] = row[1 + k];
+    for (int k = s; k < kSobolBits; k++) {
+        uint32_t m = v[k - s];
+        for (int i = 0; i < s; i++)
+            if ((p >> (s - 1 - i)) & 1u) m ^= v[k - i - 1] << (i + 1);
+        v[k] = m;
+    }
+    for (int k = 0; k < kSobolBits; k++) v[k] <<= kSobolBits - 1 - k;
+}
+
 // the (scrambled) direction numbers and shift of dimension j from its 32 random words (words 0..29: the rows of the
 // matrix, word 30: the shift); scramble = 0 gives scipy's scramble=False numbers and a zero shift
 SMCB_HD void sobol_dims(int j, int scramble, const uint32_t w[32], uint32_t sv[kSobolBits], uint32_t &shift) {
     const uint32_t full = (1u << kSobolBits) - 1u;
-    for (int k = 0; k < kSobolBits; k++) sv[k] = kSobolDirs[j][k];
+    if (j < kSobolTabDim) {
+        for (int k = 0; k < kSobolBits; k++) sv[k] = kSobolDirs[j][k];
+    } else {
+        sobol_expand(j, sv);
+    }
     shift = 0;
     if (!scramble) return;
     uint32_t rows[kSobolBits];

@@ -1,9 +1,11 @@
 """Randomised quasi-Monte Carlo points on the device (particles/rqmc.py).
 
 ``sobol(N, d)`` restates ``rqmc.sobol``: scrambled Sobol' points of ``scipy.stats.qmc.Sobol(d)`` (30 bits, a linear
-matrix scramble and a digital shift), squeezed into ``0.5 + (1 - 1e-10) * (u - 0.5)``, for d <= 32, as an (N, d) CUDA
-tensor (csrc/smcb_sqmc.cu).  The scrambling is drawn from the device Philox under a key taken from NumPy's global
-generator, so ``np.random.seed`` repeats it.  Halton and Latin hypercube points have no kernel.
+matrix scramble and a digital shift), squeezed into ``0.5 + (1 - 1e-10) * (u - 0.5)``, for d <= ``MAX_DIM`` = 4096, as
+an (N, d) CUDA tensor (csrc/smcb_sqmc.cu).  Dimension j's scrambling depends on (key, j) only, so the first k columns of
+a d-dimensional set equal the k-dimensional set of the same key.  The scrambling is drawn from the device Philox under
+a key taken from NumPy's global generator, so ``np.random.seed`` repeats it.  Halton and Latin hypercube points have no
+kernel.
 """
 import numpy as np
 import torch
@@ -12,7 +14,7 @@ from . import _lib
 from .device import context, ptr
 
 TOL = 1e-10
-MAX_DIM = 32
+MAX_DIM = 4096
 
 
 def sobol_points(N, d, seed, call=0, scramble=True, raw=False):

@@ -5,10 +5,10 @@ The reference stores references to ``smc.X / A / wgts`` (it allocates new arrays
 The device loop ping-pongs two buffers instead, so a history OWNS what it saves: ``save`` clones
 the device arrays (8(d+2) bytes per particle per saved step -- at N = 1e7 keep the window short).
 
-Backward sampling (``backward_sampling_ON2 / _mcmc / _reject``): when the transition density is a stock model's
-``PX`` (``state_space_models.transition_spec``) the whole backward pass is ONE kernel launch
-(csrc/smcb_smooth.cu); otherwise the same algorithms run with ``fk.logpt`` called on CUDA tensors, with the
-library's sampling, CDF and gather kernels underneath.  There is no CPU path.
+Backward sampling (``backward_sampling_ON2 / _mcmc / _reject / _qmc``): when the transition density is a stock
+model's ``PX`` (``state_space_models.transition_spec``) the whole backward pass is ONE kernel launch
+(csrc/smcb_smooth.cu; QMC adds the final-time draw); otherwise the same algorithms run with ``fk.logpt`` called on CUDA
+tensors, with the library's sampling, CDF and gather kernels underneath.  There is no CPU path.
 
 Two-filter smoothing (``two_filter_smoothing``, O(N^2) and O(N), one-dimensional states) works the same way:
 csrc/smcb_twofilter.cu on a stock model's transition, ``fk.logpt`` on CUDA tensors otherwise; ``smoothing_worker``
@@ -33,6 +33,15 @@ def _flat(x):
 
 def _own(x):
     return x.clone() if isinstance(x, torch.Tensor) else x
+
+
+def _np(a):
+    return a.cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+
+
+class HilbertOrdersError(NotImplementedError, ValueError):
+    """QMC backward sampling of a history that kept no Hilbert orders (not an SQMC run).  A NotImplementedError, and a
+    ValueError as the reference's ``_check_h_orders`` raises."""
 
 
 def _own_weights(w):
@@ -100,11 +109,23 @@ class RollingParticleHistory:
 
 
 class ParticleHistory(RollingParticleHistory):
-    """smoothing.py:222-270 (storage + ``extract_one_trajectory``)."""
+    """smoothing.py:222-270 (storage + ``extract_one_trajectory``).
+
+    With ``qmc`` (an SQMC run, ``SMC(qmc=True, store_history=True)``) the history also keeps ``h_orders``: at each
+    step t >= 1 ``save`` appends ``smc.h_order``, the Hilbert order of X[t-1] that the step resampled through, so that
+    ``h_orders[t]`` orders X[t] for t = 0 .. T-2 ((N,) int64 CUDA tensors, 8 more bytes per particle per step);
+    ``backward_sampling_qmc`` needs them."""
 
     def __init__(self, fk, qmc):
         self.X, self.A, self.wgts = [], [], []
+        if qmc:
+            self.h_orders = []
         self.fk = fk
+
+    def save(self, smc):
+        RollingParticleHistory.save(self, smc)
+        if hasattr(self, "h_orders") and smc.t > 0:
+            self.h_orders.append(smc.h_order)
 
     def extract_one_trajectory(self):
         traj, n = [], None
@@ -158,8 +179,24 @@ class ParticleHistory(RollingParticleHistory):
         bounds = np.array([self.fk.upper_bound_trans(t + 1) for t in range(self.T - 1)], dtype=np.float64)
         return self._backward(_lib.SMOOTH_REJECT, M, seed, noise, max_trials=max_trials, bounds=bounds)
 
-    def backward_sampling_qmc(self, M):
-        raise NotImplementedError("QMC backward sampling (of an SQMC history) is not built")
+    def backward_sampling_qmc(self, M, seed=None, noise=None):
+        """QMC forward-filtering backward-sampling of an SQMC history, smoothing.py:425-455.  One (M, T) point set u
+        (scrambled Sobol', one dimension per time, so T <= rqmc.MAX_DIM = 4096): the final draw searches u[:, T-1] in
+        the CDF of W_{T-1} taken in the Hilbert order of X[T-1]; at t < T-1 trajectory m searches u[m, t] in the CDF
+        of lw_t + logpt(t + 1, X_t, x^m_{t+1}) taken in the order ``h_orders[t]``.  ``seed`` keys the points (as
+        ``SMC(seed=)`` keys a run's), otherwise NumPy's global generator does, as ``rqmc.sobol``; ``noise={"u":
+        (M, T)}`` injects the point set.  A history without Hilbert orders raises ``HilbertOrdersError``, a
+        NotImplementedError and a ValueError."""
+        from .rqmc import MAX_DIM
+        if not hasattr(self, "h_orders"):
+            raise HilbertOrdersError("QMC backward sampling needs a history that kept the Hilbert orders of its "
+                                     "particles: run SMC(qmc=True, store_history=True)")
+        if self.T > MAX_DIM:
+            raise NotImplementedError(f"QMC backward sampling draws one Sobol' dimension per time step: T <= "
+                                      f"{MAX_DIM} (got T = {self.T})")
+        if len(self.h_orders) != self.T - 1:
+            raise ValueError(f"QMC backward sampling: {len(self.h_orders)} Hilbert orders for T = {self.T}")
+        return self._backward(_lib.SMOOTH_ON2, int(M), seed, noise, qmc=True)
 
     # ------------------------------------------------------------ two-filter
     def two_filter_smoothing(self, t, info, phi, loggamma, linear_cost=False, return_ess=False,
@@ -326,7 +363,30 @@ class ParticleHistory(RollingParticleHistory):
             _lib.check(ctx.lib.smcb_cumsum(ctx.handle, ptr(W), N, ptr(cdf[t])))
         return cdf
 
-    def _backward(self, method, M, seed, noise, nsteps=1, max_trials=0, bounds=None):
+    def _init_qmc(self, M, seed, noise):
+        """smoothing.py:443-450: the (M, T) points and idx (T, M) with the final draw idx[T-1] = hT[searchsorted(
+        cumsum(W_{T-1}[hT]), u[:, T-1])], hT the Hilbert order of X[T-1]; the search runs on the sorted column."""
+        from .hilbert import hilbert_order, hilbert_sort
+        from .rqmc import sobol_points
+        T, dev = self.T, self.X[-1].device
+        ctx = context(dev)
+        if noise is not None and noise.get("u") is not None:
+            u = as_device(noise["u"], device=dev).reshape(M, T)
+        else:
+            key = int(np.random.randint(0, 2 ** 62, dtype=np.int64)) if seed is None else int(seed)
+            u = sobol_points(M, T, key).t()
+        orders = [as_device(h, dtype=torch.int64, device=dev).reshape(-1) for h in self.h_orders]
+        hT = hilbert_sort(self.X[-1])
+        cdf = rs.cumsum(self.wgts[-1].W[hT])
+        uT = u[:, T - 1].contiguous()
+        tau = hilbert_order(uT)                                  # argsort: the search takes sorted queries
+        found = torch.empty(M, dtype=torch.int64, device=dev)
+        _lib.check(ctx.lib.smcb_searchsorted(ctx.handle, ptr(cdf), cdf.shape[0], ptr(uT[tau]), M, ptr(found)))
+        idx = torch.empty((T, M), dtype=torch.int64, device=dev)
+        idx[-1, tau] = hT[found]
+        return u, orders, idx
+
+    def _backward(self, method, M, seed, noise, nsteps=1, max_trials=0, bounds=None, qmc=False):
         if M < 1:
             raise ValueError("backward sampling: M must be >= 1")
         from .state_space_models import transition_spec
@@ -334,9 +394,14 @@ class ParticleHistory(RollingParticleHistory):
         if seed is not None:
             ctx.seed(seed)
         spec = transition_spec(self.fk)
-        idx = self._init_backward_sampling(M, noise)
+        orders = None
+        if qmc:
+            u, orders, idx = self._init_qmc(M, seed, noise)
+            noise = {"u": u[:, :self.T - 1]}
+        else:
+            idx = self._init_backward_sampling(M, noise)
         if spec is None:
-            idx = self._plugin(method, M, idx, noise, nsteps, max_trials, bounds)
+            idx = self._plugin(method, M, idx, noise, nsteps, max_trials, bounds, orders)
         d, keep, Xs = self._history_desc(method if spec is not None else _lib.SMOOTH_GATHER, M)
         dev = Xs[0].device
         T, N, D = self.T, d.N, d.dim
@@ -353,8 +418,12 @@ class ParticleHistory(RollingParticleHistory):
             d.nsteps, d.max_trials = nsteps, max_trials
             nz = noise or {}
             if method == _lib.SMOOTH_ON2 and nz.get("u") is not None:
-                keep["u"] = as_device(np.asarray(nz["u"]).reshape(M, T - 1), device=dev)
+                keep["u"] = as_device(nz["u"], device=dev).reshape(M, T - 1).contiguous()
                 d.u = keep["u"].data_ptr()
+            if orders and T > 1:
+                keep["orders"] = orders
+                keep["tord"] = torch.tensor([o.data_ptr() for o in orders], dtype=torch.int64, device=dev)
+                d.order = keep["tord"].data_ptr()
             if method != _lib.SMOOTH_ON2:
                 if nz.get("prop") is not None:
                     shape = (T - 1, nsteps, M) if method == _lib.SMOOTH_MCMC else (T - 1, M, max_trials)
@@ -382,17 +451,20 @@ class ParticleHistory(RollingParticleHistory):
         return self._output_backward_sampling(paths)
 
     # ----------------------------------------------------------- plugin path
-    def _exact_draw(self, t, xn, u, out):
+    def _exact_draw(self, t, xn, u, out, order=None):
         """smoothing.py:310 / 418-421 for one trajectory: searchsorted(cumsum(exp_and_normalise(lw_t +
-        logpt(t + 1, X_t, xn))), u) written into the device int64 scalar ``out``."""
+        logpt(t + 1, X_t, xn))), u) written into the device int64 scalar ``out``.  With ``order`` (QMC, smoothing.py:
+        449-452) the CDF runs over the weights in that order and the position found maps back through it."""
         ctx = context(out.device)
         W = rs.exp_and_normalise(self.wgts[t].lw + as_device(self.fk.logpt(t + 1, self.X[t], xn)))
-        cdf = rs.cumsum(W)
+        cdf = rs.cumsum(W if order is None else W[order])
         su = rs._uniforms(1, W) if u is None else torch.full((1,), float(u), dtype=torch.float64, device=W.device)
         _lib.check(ctx.lib.smcb_searchsorted(ctx.handle, ptr(cdf), W.shape[0], ptr(su), 1, C.c_void_p(out.data_ptr())))
         out.masked_fill_(~(W.sum() > 0), 0)      # no positive weight (a NaN row): 0, as the kernels' exact draws
+        if order is not None:
+            out.copy_(order[out])
 
-    def _plugin(self, method, M, idx, noise, nsteps, max_trials, bounds):
+    def _plugin(self, method, M, idx, noise, nsteps, max_trials, bounds, orders=None):
         """The reference's loops with ``fk.logpt`` on CUDA tensors (vectorised over M for MCMC / reject, over N per
         (t, m) for ON2); indices stay on the device."""
         nz = noise or {}
@@ -400,11 +472,12 @@ class ParticleHistory(RollingParticleHistory):
         dev = idx.device
         X = self.X
         if method == _lib.SMOOTH_ON2:
-            u = None if nz.get("u") is None else np.asarray(nz["u"]).reshape(M, T - 1)
+            u = None if nz.get("u") is None else _np(nz["u"]).reshape(M, T - 1)
             for m in range(M):
                 for t in reversed(range(T - 1)):
                     xn = X[t + 1][idx[t + 1, m]]
-                    self._exact_draw(t, xn, None if u is None else u[m, t], idx[t, m])
+                    self._exact_draw(t, xn, None if u is None else u[m, t], idx[t, m],
+                                     None if orders is None else orders[t])
             return idx
         if method == _lib.SMOOTH_MCMC:
             prop_in = None if nz.get("prop") is None else as_device(np.asarray(nz["prop"]).reshape(T - 1, nsteps, M),
@@ -472,15 +545,19 @@ def smoothing_worker(method=None, N=100, fk=None, fk_info=None, add_func=None, l
     Returns {"est": (T-1,) array, "cpu": seconds}: the estimates stay on the device until one read at the end, and
     ``cpu`` is the wall time of the runs plus the smoothing, ending with that read.  'FFBS_purereject' is the
     hybrid sampler with 2^24 - 1 proposals per draw before the exact draw (the reference allows N * 10^9);
-    'FFBS_QMC' raises NotImplementedError (QMC backward sampling of an SQMC history is not built); an unknown method raises ValueError."""
+    'FFBS_QMC' raises NotImplementedError: it needs an SQMC forward pass, and the reference's worker calls
+    ``particles.SQMC``, which the reference does not define, so there is no behaviour to follow; run
+    ``SMC(qmc=True, store_history=True)`` and then ``hist.backward_sampling_qmc`` instead.  An unknown method raises
+    ValueError."""
     import time
 
     from .core import SMC
     if method not in WORKER_METHODS:
         raise ValueError(f"smoothing_worker: no such method {method!r}; one of {WORKER_METHODS}")
     if method == "FFBS_QMC":
-        raise NotImplementedError("smoothing_worker: FFBS_QMC needs QMC backward sampling of an SQMC history, "
-                                  "which is not built")
+        raise NotImplementedError("smoothing_worker: FFBS_QMC needs an SQMC forward pass, which the reference's "
+                                  "worker asks of particles.SQMC, a class it does not define; run SMC(qmc=True, "
+                                  "store_history=True) and then hist.backward_sampling_qmc(M)")
     T = fk.T
     if fk_info is None:
         fk_info = fk.__class__(ssm=fk.ssm, data=fk.data[::-1])
