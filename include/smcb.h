@@ -115,15 +115,6 @@ int smcb_gather_rows(smcb_ctx *ctx, const double *X, int64_t n, const int64_t *A
 /* Normal.rvs, distributions.py:270-271; z_in = injected N(0,1) draws or NULL */
 int smcb_normal_rvs(smcb_ctx *ctx, const double *loc, double loc0, const double *scale,
                     double scale0, const double *z_in, double *out, int64_t n);
-/* Normal.logpdf, distributions.py:273-274 */
-int smcb_normal_logpdf(smcb_ctx *ctx, const double *x, double x0, const double *loc,
-                       double loc0, const double *scale, double scale0, double *out,
-                       int64_t n);
-/* other univariate log-densities (distributions.py): kind 0 Student(df = p0, loc, scale) :417-433, 1 Gamma(a = p0,
- * rate) :336-356, 2 Laplace(loc, scale) :399-414, 3 Logistic(loc, scale) :381-396; p1 / p2 arrays or scalars as for
- * Normal; c0 = the host-computed lgamma constant of the density (0 for kinds 2, 3) */
-int smcb_logpdf1(smcb_ctx *ctx, int kind, const double *x, double x0, double p0, double c0, const double *p1,
-                 double p10, const double *p2, double p20, double *out, int64_t n);
 /* MvNormal.rvs / logpdf, distributions.py:946-969; SoA (d, n), d <= 32; L = host (d,d) lower
  * Cholesky factor of cov, row-major; loc/scale: array (d, n), or NULL + host vector[d].
  * d <= 8: factor in the kernel parameters, two particles per thread; 8 < d <= 32: factor in shared
@@ -138,7 +129,7 @@ int smcb_mvnormal_logpdf(smcb_ctx *ctx, const double *x, const double *loc,
 int smcb_standard_normal(smcb_ctx *ctx, double *out, int64_t n);
 int smcb_uniform(smcb_ctx *ctx, double *out, int64_t n);
 
-/* The laws of distributions.py with a kernel of their own (csrc/smcb_dists.cuh), by law code:
+/* The univariate laws of distributions.py with a device log-density (csrc/smcb_dists.cuh), by law code:
  *   0 InvGamma(a, b)                  :358-377  scipy.stats.invgamma.logpdf(x, a, scale=b); draws b / Gamma(a, 1)
  *   1 LogNormal(mu, sigma)            :379-396  scipy.stats.lognorm.logpdf(x, sigma, scale=exp(mu))
  *   2 TruncNormal(mu, sigma, a, b)    :475-505  scipy.stats.truncnorm.logpdf, mass in log space; exact draws
@@ -146,11 +137,19 @@ int smcb_uniform(smcb_ctx *ctx, double *out, int64_t n);
  *   4 Geometric(p)                    :552-565  scipy.stats.geom.logpmf (support 1, 2, ...)
  *   5 NegativeBinomial(n, p)          :568-595  scipy.stats.nbinom.logpmf(x, n, p), the law its draws follow
  *   6 DiscreteUniform(lo, hi)         :631-649  -log(hi - lo) on lo .. hi - 1
- *   7 Gamma(a, rate b)                draws only: the sampler InvGamma, NegativeBinomial and Dirichlet draw through
+ *   7 Gamma(a, rate b, c0)            :336-356  scipy.stats.gamma.logpdf(x, a, scale=1/b), c0 = -gammaln(a); the
+ *                                               sampler InvGamma, NegativeBinomial and Dirichlet draw through
+ *                                               (c0 unused)
+ *   8 Normal(loc, scale)              :267-285  scipy.stats.norm.logpdf
+ *   9 Student(df, loc, scale, c0)     :417-433  scipy.stats.t.logpdf, c0 = gammaln((df + 1) / 2) - gammaln(df / 2)
+ *                                               - log(df pi) / 2
+ *  10 Laplace(loc, scale)             :301-314  scipy.stats.laplace.logpdf
+ *  11 Logistic(loc, scale)            :288-299  scipy.stats.logistic.logpdf
  * Parameter k is the array pk of n values, or NULL and the scalar s[k] (s: host array of 4 doubles; unused ones
- * are ignored).  NaN outside a law's parameter domain, -inf outside its support and, for codes 3-6, at non-integer
- * x.  Draws: fp64 into out for codes 0-2 and 7, int64 for the discrete codes 3-6 (INT64_MIN where a parameter is
- * outside its domain); element i's draw depends on (seed, API call, i) only. */
+ * are ignored).  For codes 0-6, NaN outside a law's parameter domain, -inf outside its support and, for codes 3-6,
+ * at non-integer x.  smcb_dist_rvs takes codes 0-7 (codes 8-11 draw through smcb_normal_rvs or outside the library):
+ * fp64 into out for codes 0-2 and 7, int64 for the discrete codes 3-6 (INT64_MIN where a parameter is outside its
+ * domain); element i's draw depends on (seed, API call, i) only. */
 int smcb_dist_logpdf(smcb_ctx *ctx, int law, const double *x, double x0, const double *p0, const double *p1,
                      const double *p2, const double *p3, const double *s, double *out, int64_t n);
 int smcb_dist_rvs(smcb_ctx *ctx, int law, const double *p0, const double *p1, const double *p2, const double *p3,

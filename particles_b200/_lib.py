@@ -22,7 +22,8 @@ MODEL_BEARINGS, MODEL_MVLINGAUSS, MODEL_DISCRETECOX, MODEL_STOCHVOLLEV = 4, 5, 6
 LSE_SUM, LSE_MEAN, LSE_ESSL = 0, 1, 2
 # law codes of smcb_dist_logpdf / smcb_dist_rvs
 LAW_INVGAMMA, LAW_LOGNORMAL, LAW_TRUNCNORMAL, LAW_BINOMIAL, LAW_GEOMETRIC = 0, 1, 2, 3, 4
-LAW_NEGBINOMIAL, LAW_DISCRETEUNIFORM, LAW_GAMMA = 5, 6, 7
+LAW_NEGBINOMIAL, LAW_DISCRETEUNIFORM, LAW_GAMMA, LAW_NORMAL, LAW_STUDENT = 5, 6, 7, 8, 9
+LAW_LAPLACE, LAW_LOGISTIC = 10, 11
 # bits of smcb_dirichlet_logpdf's *bad: the tests of scipy.stats.dirichlet's input check
 DIRICHLET_RANGE, DIRICHLET_ZERO, DIRICHLET_SUM, DIRICHLET_NAN = 1, 2, 4, 8
 
@@ -220,10 +221,6 @@ PROTOTYPES = {
     "smcb_gather": (C.c_int, [C.c_void_p, c_dp, C.c_int64, c_dp, C.c_int64, C.c_int, c_dp]),
     "smcb_gather_rows": (C.c_int, [C.c_void_p, c_dp, C.c_int64, c_dp, C.c_int64, C.c_int, c_dp]),
     "smcb_normal_rvs": (C.c_int, [C.c_void_p, c_dp, C.c_double, c_dp, C.c_double, c_dp, c_dp, C.c_int64]),
-    "smcb_normal_logpdf": (C.c_int, [C.c_void_p, c_dp, C.c_double, c_dp, C.c_double, c_dp, C.c_double,
-                                     c_dp, C.c_int64]),
-    "smcb_logpdf1": (C.c_int, [C.c_void_p, C.c_int, c_dp, C.c_double, C.c_double, C.c_double, c_dp, C.c_double, c_dp,
-                               C.c_double, c_dp, C.c_int64]),
     "smcb_mvnormal_rvs": (C.c_int, [C.c_void_p, c_dp, c_dp, c_dp, c_dp, c_dp, C.c_int, c_dp, c_dp, C.c_int64]),
     "smcb_mvnormal_logpdf": (C.c_int, [C.c_void_p, c_dp, c_dp, c_dp, c_dp, c_dp, c_dp, C.c_int, c_dp,
                                        C.c_int64]),

@@ -857,69 +857,12 @@ __global__ void __launch_bounds__(kBlock) k_normal_rvs(Philox key, uint64_t call
     }
 }
 
-__global__ void __launch_bounds__(kBlock) k_normal_logpdf(const double *__restrict__ x, double x0,
-                                                         const double *__restrict__ loc, double loc0,
-                                                         const double *__restrict__ scale, double scale0,
-                                                         double *__restrict__ out, int64_t n) {
-    const int64_t stride = (int64_t)gridDim.x * kBlock;
-    for (int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x; i < n; i += stride)
-        out[i] = normal_logpdf(x ? x[i] : x0, loc ? loc[i] : loc0, scale ? scale[i] : scale0);
-}
-
 extern "C" int smcb_normal_rvs(smcb_ctx *c, const double *loc, double loc0, const double *scale,
                                double scale0, const double *z_in, double *out, int64_t n) {
     SMCB_REQUIRE(c && out && n >= 1, "smcb_normal_rvs: bad argument");
     uint64_t call = z_in ? 0 : c->api_counter++;
     return launch(c, k_normal_rvs, grid_for((n + 1) / 2, kBlock * 4), kBlock, 0, key_of(c->seed), call, loc, loc0,
                   scale, scale0, z_in, out, n);
-}
-
-extern "C" int smcb_normal_logpdf(smcb_ctx *c, const double *x, double x0, const double *loc,
-                                  double loc0, const double *scale, double scale0, double *out,
-                                  int64_t n) {
-    SMCB_REQUIRE(c && out && n >= 1, "smcb_normal_logpdf: bad argument");
-    return launch(c, k_normal_logpdf, grid_for(n, kBlock * 4), kBlock, 0, x, x0, loc, loc0, scale, scale0, out, n);
-}
-
-// ---------------------------------------------------------------------------
-// more univariate log-densities of distributions.py (the ones a state-space model's PY / PX may use): one
-// elementwise kernel, parameters scalar or per-particle arrays as for Normal.
-//   kind 0 Student(df, loc, scale)  distributions.py:417-433  (scipy.stats.t.logpdf)
-//   kind 1 Gamma(a, b)              distributions.py:336-356  (scipy.stats.gamma.logpdf(x, a, scale = 1 / b))
-//   kind 2 Laplace(loc, scale)      distributions.py:399-414
-//   kind 3 Logistic(loc, scale)     distributions.py:381-396
-// p0 is a scalar (df resp. a); its lgamma terms come in as host-computed constants c0.
-// ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(kBlock) k_logpdf1(int kind, const double *__restrict__ x, double x0, double p0, double c0,
-                                                   const double *__restrict__ p1, double p10,
-                                                   const double *__restrict__ p2, double p20,
-                                                   double *__restrict__ out, int64_t n) {
-    const int64_t stride = (int64_t)gridDim.x * kBlock;
-    for (int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x; i < n; i += stride) {
-        const double xv = x ? x[i] : x0, a = p1 ? p1[i] : p10, b = p2 ? p2[i] : p20;
-        double r;
-        if (kind == 0) {                  // c0 = gammaln((df+1)/2) - gammaln(df/2) - log(df pi)/2
-            const double z = (xv - a) / b;
-            r = c0 - 0.5 * (p0 + 1.0) * log1p(z * z / p0) - log(b);
-        } else if (kind == 1) {           // a = rate b (array or scalar); c0 = -gammaln(a_shape)
-            // scipy's xlogy(a - 1, x): the term is 0 when a == 1, also at x = 0 and x = +inf; at x = 0 it is +inf for
-            // a < 1 and -inf for a > 1, and x = +inf gives -inf for a <= 1 and NaN (inf - inf) for a > 1
-            const double xl = (p0 == 1.0) ? 0.0 : (p0 - 1.0) * log(xv);
-            r = (xv != xv) ? xv : (xv >= 0.0) ? p0 * log(a) + c0 + xl - a * xv : -CUDART_INF;
-        } else if (kind == 2) {
-            r = -log(2.0 * b) - fabs(xv - a) / b;
-        } else {                          // scipy's symmetric form: exp(-|z|) cannot overflow
-            const double y = -fabs((xv - a) / b);
-            r = y - 2.0 * log1p(exp(y)) - log(b);
-        }
-        out[i] = r;
-    }
-}
-
-extern "C" int smcb_logpdf1(smcb_ctx *c, int kind, const double *x, double x0, double p0, double c0, const double *p1,
-                            double p10, const double *p2, double p20, double *out, int64_t n) {
-    SMCB_REQUIRE(c && out && n >= 1 && kind >= 0 && kind <= 3, "smcb_logpdf1: bad argument");
-    return launch(c, k_logpdf1, grid_for(n, kBlock * 4), kBlock, 0, kind, x, x0, p0, c0, p1, p10, p2, p20, out, n);
 }
 
 constexpr int kMaxDim = 8;

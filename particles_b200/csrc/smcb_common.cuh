@@ -214,13 +214,6 @@ __device__ __forceinline__ Lse3 lse3_block_reduce(Lse3 a, Lse3 *smem /* BLOCK/32
     return a;
 }
 
-// Normal.logpdf, distributions.py:273-274 (scipy.stats.norm.logpdf): the operation
-// order of SURVEY.md section 9 item 2
-__device__ __forceinline__ double normal_logpdf(double x, double loc, double scale) {
-    double z = (x - loc) / scale;
-    return -z * z / 2.0 - kHalfLog2Pi - log(scale);
-}
-
 // streaming 16-byte accesses (two fp64 particles per thread)
 __device__ __forceinline__ double2 ld2(const double *p) {
     return *reinterpret_cast<const double2 *>(p);

@@ -1,8 +1,9 @@
-// smcb_dists.cuh -- log-densities and samplers of the laws of distributions.py that have no kernel elsewhere:
-// InvGamma, LogNormal, TruncNormal, Binomial, Geometric, NegativeBinomial, DiscreteUniform, and the Gamma sampler
-// that InvGamma, NegativeBinomial and Dirichlet draw through.  Every function is __host__ __device__: the library's
-// kernels (smcb_dists.cu) and the CPU harness of the tests (tests/dists_host.cpp, g++ -ffp-contract=off) compile
-// this same header, so the host build's draws replay the device's from the same Philox counters.
+// smcb_dists.cuh -- the device log-densities of the univariate laws of distributions.py, and the samplers of those
+// whose draws come from here: InvGamma, LogNormal, TruncNormal, Binomial, Geometric, NegativeBinomial,
+// DiscreteUniform and Gamma (the sampler InvGamma, NegativeBinomial and Dirichlet draw through) have both; Normal,
+// Student, Laplace and Logistic have their log-density here and draw elsewhere.  Every function is
+// __host__ __device__: the library's kernels (smcb_dists.cu) and the CPU harness of the tests (tests/dists_host.cpp,
+// g++ -ffp-contract=off) compile this same header, so the host build replays the device's values and draws.
 //
 // Randomness: the draw of element i reads Philox blocks with counter (i lo, block, call lo, (i hi << 8) | purpose)
 // under the context's key, `call` = the API call number.  A rejection sampler's k-th trial always reads the same
@@ -18,12 +19,13 @@ namespace dists {
 
 #define SMCB_HD __host__ __device__ __forceinline__
 
-// law codes (include/smcb.h, distributions.py)
+// law codes (include/smcb.h, distributions.py); the codes below kNumSampled have a sampler here
 enum : int {
     kInvGamma = 0, kLogNormal = 1, kTruncNormal = 2, kBinomial = 3, kGeometric = 4, kNegBinomial = 5,
-    kDiscreteUniform = 6, kGamma = 7, kNumLaws = 8,
+    kDiscreteUniform = 6, kGamma = 7, kNormal = 8, kStudent = 9, kLaplace = 10, kLogistic = 11, kNumLaws = 12,
+    kNumSampled = 8,
 };
-SMCB_HD bool discrete_law(int law) { return law >= kBinomial && law <= kDiscreteUniform; }
+SMCB_HD constexpr bool discrete_law(int law) { return law >= kBinomial && law <= kDiscreteUniform; }
 
 constexpr double kLogSqrt2Pi = 0.91893853320467274178;   // log(2 pi) / 2
 constexpr double kLog2Pi = 1.8378770664093454836;
@@ -221,6 +223,39 @@ SMCB_HD double discrete_uniform_logpmf(double x, double lo, double hi) {
     return -log(hi - lo);
 }
 
+// The laws of state-space models' PX / PY: scipy's formulas without its parameter checks.  Their lgamma terms come
+// from the host as c0 (scipy's gammaln), not from the device's lgamma.
+// scipy.stats.norm.logpdf(x, loc, scale), in the operation order of SURVEY.md section 9 item 2
+SMCB_HD double normal_logpdf(double x, double loc, double scale) {
+    const double z = (x - loc) / scale;
+    return -z * z / 2.0 - kLogSqrt2Pi - log(scale);
+}
+
+// scipy.stats.t.logpdf(x, df, loc, scale); c0 = gammaln((df + 1) / 2) - gammaln(df / 2) - log(df pi) / 2
+SMCB_HD double student_logpdf(double x, double df, double loc, double scale, double c0) {
+    const double z = (x - loc) / scale;
+    return c0 - 0.5 * (df + 1.0) * log1p(z * z / df) - log(scale);
+}
+
+// scipy.stats.gamma.logpdf(x, a, scale=1 / b); c0 = -gammaln(a).  scipy's xlogy(a - 1, x): the term is 0 when
+// a == 1, also at x = 0 and x = +inf; at x = 0 it is +inf for a < 1 and -inf for a > 1, and x = +inf gives -inf for
+// a <= 1 and NaN (inf - inf) for a > 1
+SMCB_HD double gamma_logpdf(double x, double a, double b, double c0) {
+    const double xl = (a == 1.0) ? 0.0 : (a - 1.0) * log(x);
+    return (x != x) ? x : (x >= 0.0) ? a * log(b) + c0 + xl - b * x : -inf_();
+}
+
+// scipy.stats.laplace.logpdf(x, loc, scale)
+SMCB_HD double laplace_logpdf(double x, double loc, double scale) {
+    return -log(2.0 * scale) - fabs(x - loc) / scale;
+}
+
+// scipy.stats.logistic.logpdf(x, loc, scale) in scipy's symmetric form: exp(-|z|) cannot overflow
+SMCB_HD double logistic_logpdf(double x, double loc, double scale) {
+    const double y = -fabs((x - loc) / scale);
+    return y - 2.0 * log1p(exp(y)) - log(scale);
+}
+
 SMCB_HD double law_logpdf(int law, double x, double p0, double p1, double p2, double p3) {
     switch (law) {
         case kInvGamma: return invgamma_logpdf(x, p0, p1);
@@ -229,7 +264,12 @@ SMCB_HD double law_logpdf(int law, double x, double p0, double p1, double p2, do
         case kBinomial: return binomial_logpmf(x, p0, p1);
         case kGeometric: return geometric_logpmf(x, p0);
         case kNegBinomial: return nbinom_logpmf(x, p0, p1);
-        default: return discrete_uniform_logpmf(x, p0, p1);
+        case kDiscreteUniform: return discrete_uniform_logpmf(x, p0, p1);
+        case kGamma: return gamma_logpdf(x, p0, p1, p2);
+        case kNormal: return normal_logpdf(x, p0, p1);
+        case kStudent: return student_logpdf(x, p0, p1, p2, p3);
+        case kLaplace: return laplace_logpdf(x, p0, p1);
+        default: return logistic_logpdf(x, p0, p1);
     }
 }
 

@@ -32,6 +32,8 @@ def _split(v):
     """scalar-or-array argument -> (device tensor or None, scalar).  A size-1 array or tensor is a scalar that
     broadcasts -- ``StateSpaceModel.simulate`` returns observations of shape (1,), and NumPy broadcasts
     ``data[t]`` against the (N,) particles (SURVEY.md section 9.10)."""
+    if isinstance(v, (int, float)):                     # numpy.float64 too
+        return None, float(v)
     if isinstance(v, torch.Tensor):
         if v.numel() == 1:
             return None, float(v.reshape(-1)[0].item())
@@ -69,24 +71,66 @@ class LocScaleDist(ProbDist):
         self.scale = scale
 
 
-class Normal(LocScaleDist):
-    """N(loc, scale^2) -- particles/distributions.py:267-285."""
+def _common_length(size, *arrs):
+    """Common length of the array arguments (scalars broadcast); mismatched lengths are an error, as NumPy's
+    broadcasting would make them."""
+    lens = {int(a.shape[0]) for a in arrs if a is not None}
+    if len(lens) > 1:
+        raise ValueError(f"operands could not be broadcast together with lengths {sorted(lens)}")
+    if lens:
+        return lens.pop()
+    return 1 if size is None else int(size)
 
-    def _n(self, size, *arrs):
-        """Common length of the array arguments (scalars broadcast); mismatched lengths are an error, as NumPy's
-        broadcasting would make them."""
-        lens = {int(a.shape[0]) for a in arrs if a is not None}
-        if len(lens) > 1:
-            raise ValueError(f"operands could not be broadcast together with lengths {sorted(lens)}")
-        if lens:
-            return lens.pop()
-        return 1 if size is None else int(size)
+
+class _KernelLaw(ProbDist):
+    """A law with a device log-density, law code ``_law`` of include/smcb.h, and, for codes 0-7, a device sampler.
+    Its parameters, ``_params()``, are scalars or (N,) arrays / tensors: array parameters make it a Markov kernel,
+    as in the reference (distributions.py:135-154)."""
+    _law = None
+
+    def _params(self):
+        raise NotImplementedError
+
+    def _args(self):
+        """-> the four parameters' device arrays (None for a scalar) and the host array of their scalars"""
+        arrays, scalars = [None] * 4, (C.c_double * 4)()
+        for k, v in enumerate(self._params()):
+            arrays[k], scalars[k] = _split(v)
+        return arrays, scalars
+
+    def logpdf(self, x):
+        xa, x0 = _split(x)
+        arrays, scalars = self._args()
+        n = _common_length(None, xa, *arrays)
+        ctx = context()
+        out = empty(n)
+        _lib.check(ctx.lib.smcb_dist_logpdf(ctx.handle, self._law, ptr(xa), x0, *map(ptr, arrays), scalars,
+                                            ptr(out), n))
+        return out
+
+    def rvs(self, size=None):
+        arrays, scalars = self._args()
+        n = _common_length(size, *arrays)
+        if size is not None and int(size) != n:        # numpy.random's broadcast error
+            raise ValueError(f"shape mismatch: {n} parameter values cannot be broadcast to size {int(size)}")
+        ctx = context()
+        out = empty(n, dtype=torch.int64 if self.dtype == np.int64 else torch.float64)
+        _lib.check(ctx.lib.smcb_dist_rvs(ctx.handle, self._law, *map(ptr, arrays), scalars, ptr(out), n))
+        return out
+
+
+class Normal(LocScaleDist, _KernelLaw):
+    """N(loc, scale^2) -- particles/distributions.py:267-285."""
+    _law = _lib.LAW_NORMAL
+
+    def _params(self):
+        return self.loc, self.scale
 
     def rvs(self, size=None, z=None):
         la, l0 = _split(self.loc)
         sa, s0 = _split(self.scale)
         zd = None if z is None else as_device(z)
-        n = self._n(size, la, sa, zd)
+        n = _common_length(size, la, sa, zd)
         ctx = context()
         out = empty(n)
         _lib.check(ctx.lib.smcb_normal_rvs(ctx.handle, ptr(la), l0, ptr(sa), s0, ptr(zd), ptr(out), n))
@@ -95,17 +139,6 @@ class Normal(LocScaleDist):
     def ppf(self, u):
         """scipy.stats.norm.ppf(u, loc, scale) = loc + scale * Phi^-1(u), on the device."""
         return self.rvs(z=ndtri(u))
-
-    def logpdf(self, x):
-        xa, x0 = _split(x)
-        la, l0 = _split(self.loc)
-        sa, s0 = _split(self.scale)
-        n = self._n(None, xa, la, sa)
-        ctx = context()
-        out = empty(n)
-        _lib.check(ctx.lib.smcb_normal_logpdf(ctx.handle, ptr(xa), x0, ptr(la), l0, ptr(sa), s0,
-                                              ptr(out), n))
-        return out
 
     def posterior(self, x, sigma=1.0):
         """particles/distributions.py:279-285: X_1..X_n ~ N(theta, sigma^2), theta ~ self (host arithmetic)."""
@@ -117,62 +150,42 @@ class Normal(LocScaleDist):
         return Normal(loc=mu, scale=np.sqrt(varp))
 
 
-class _Univariate(ProbDist):
-    """logpdf through the elementwise kernel smcb_logpdf1 (kinds: 0 Student, 1 Gamma, 2 Laplace, 3 Logistic)."""
-    _kind = None
-
-    def _call(self, x, p0, c0, a, b):
-        xa, x0 = _split(x)
-        aa, a0 = _split(a)
-        ba, b0 = _split(b)
-        lens = {int(v.shape[0]) for v in (xa, aa, ba) if v is not None}
-        if len(lens) > 1:
-            raise ValueError(f"operands could not be broadcast together with lengths {sorted(lens)}")
-        n = lens.pop() if lens else 1
-        ctx = context()
-        out = empty(n)
-        _lib.check(ctx.lib.smcb_logpdf1(ctx.handle, self._kind, ptr(xa), x0, float(p0), float(c0), ptr(aa), a0,
-                                        ptr(ba), b0, ptr(out), n))
-        return out
-
-
-class Student(_Univariate):
+class Student(_KernelLaw):
     """Student(df, loc, scale) -- particles/distributions.py:417-433 (scipy.stats.t.logpdf); ``df`` scalar."""
-    _kind = 0
+    _law = _lib.LAW_STUDENT
 
     def __init__(self, df=3.0, loc=0.0, scale=1.0):
         self.df, self.loc, self.scale = df, loc, scale
 
-    def logpdf(self, x):
+    def _params(self):
         from scipy.special import gammaln
         df = float(self.df)
-        c0 = gammaln(0.5 * (df + 1.0)) - gammaln(0.5 * df) - 0.5 * np.log(df * np.pi)
-        return self._call(x, df, c0, self.loc, self.scale)
+        return df, self.loc, self.scale, gammaln(0.5 * (df + 1.0)) - gammaln(0.5 * df) - 0.5 * np.log(df * np.pi)
 
     def rvs(self, size=None):
         """loc + scale * z / sqrt(chi2_df / df): the normals from the context's Philox stream, the chi-square
         from torch's generator (the reference draws through scipy.stats.t.rvs)."""
         la, l0 = _split(self.loc)
         sa, s0 = _split(self.scale)
-        n = la.shape[0] if la is not None else (sa.shape[0] if sa is not None else (1 if size is None else int(size)))
+        n = _common_length(size, la, sa)
         z = Normal().rvs(size=n)
         g = torch.distributions.Chi2(torch.tensor(float(self.df), dtype=torch.float64, device=z.device)).sample((n,))
         t = z / torch.sqrt(g / float(self.df))
         return (la if la is not None else l0) + (sa if sa is not None else s0) * t
 
 
-class Gamma(_Univariate):
+class Gamma(_KernelLaw):
     """Gamma(a, b), density prop. to x^(a-1) exp(-b x) -- particles/distributions.py:336-356; ``a`` scalar,
     ``b`` scalar or per-particle array."""
-    _kind = 1
+    _law = _lib.LAW_GAMMA
 
     def __init__(self, a=1.0, b=1.0):
         self.a, self.b = a, b
         self.scale = 1.0 / b
 
-    def logpdf(self, x):
+    def _params(self):
         from scipy.special import gammaln
-        return self._call(x, float(self.a), -gammaln(float(self.a)), self.b, 1.0)
+        return float(self.a), self.b, -gammaln(float(self.a))
 
     def posterior(self, x):
         """particles/distributions.py:353-355: X_1..X_n ~ N(0, 1/theta), theta ~ self."""
@@ -186,32 +199,32 @@ class Gamma(_Univariate):
         return torch.distributions.Gamma(a, b).sample()
 
 
-class Laplace(LocScaleDist, _Univariate):
+class Laplace(LocScaleDist, _KernelLaw):
     """particles/distributions.py:301-314."""
-    _kind = 2
+    _law = _lib.LAW_LAPLACE
 
-    def logpdf(self, x):
-        return self._call(x, 0.0, 0.0, self.loc, self.scale)
+    def _params(self):
+        return self.loc, self.scale
 
     def rvs(self, size=None):
         la, l0 = _split(self.loc)
         sa, s0 = _split(self.scale)
-        n = la.shape[0] if la is not None else (sa.shape[0] if sa is not None else (1 if size is None else int(size)))
+        n = _common_length(size, la, sa)
         u = torch.rand(n, dtype=torch.float64, device="cuda") - 0.5
         return (la if la is not None else l0) - (sa if sa is not None else s0) * torch.sign(u) * torch.log1p(-2 * u.abs())
 
 
-class Logistic(LocScaleDist, _Univariate):
+class Logistic(LocScaleDist, _KernelLaw):
     """particles/distributions.py:288-299."""
-    _kind = 3
+    _law = _lib.LAW_LOGISTIC
 
-    def logpdf(self, x):
-        return self._call(x, 0.0, 0.0, self.loc, self.scale)
+    def _params(self):
+        return self.loc, self.scale
 
     def rvs(self, size=None):
         la, l0 = _split(self.loc)
         sa, s0 = _split(self.scale)
-        n = la.shape[0] if la is not None else (sa.shape[0] if sa is not None else (1 if size is None else int(size)))
+        n = _common_length(size, la, sa)
         u = torch.rand(n, dtype=torch.float64, device="cuda")
         return (la if la is not None else l0) + (sa if sa is not None else s0) * (torch.log(u) - torch.log1p(-u))
 
@@ -547,53 +560,8 @@ class MvNormal(ProbDist):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# laws of the elementwise kernels smcb_dist_logpdf / smcb_dist_rvs (csrc/smcb_dists.cuh)
+# laws with a device sampler in csrc/smcb_dists.cuh (smcb_dist_rvs)
 # ---------------------------------------------------------------------------------------------------------------------
-def _common_length(size, *arrs):
-    lens = {int(a.shape[0]) for a in arrs if a is not None}
-    if len(lens) > 1:
-        raise ValueError(f"operands could not be broadcast together with lengths {sorted(lens)}")
-    if lens:
-        return lens.pop()
-    return 1 if size is None else int(size)
-
-
-class _KernelLaw(ProbDist):
-    """A law with a device log-density and sampler (law code ``_law`` of include/smcb.h).  Its parameters,
-    ``_params()``, are scalars or (N,) arrays / tensors: array parameters make it a Markov kernel, as for Normal."""
-    _law = None
-
-    def _params(self):
-        raise NotImplementedError
-
-    def _args(self):
-        ps = [_split(v) for v in self._params()]
-        arrays = [a for a, _ in ps] + [None] * (4 - len(ps))
-        scalars = np.array([v for _, v in ps] + [0.0] * (4 - len(ps)), dtype=np.float64)
-        return arrays, scalars
-
-    def logpdf(self, x):
-        xa, x0 = _split(x)
-        arrays, scalars = self._args()
-        n = _common_length(None, xa, *arrays)
-        ctx = context()
-        out = empty(n)
-        _lib.check(ctx.lib.smcb_dist_logpdf(ctx.handle, self._law, ptr(xa), x0, *[ptr(a) for a in arrays],
-                                            scalars.ctypes.data_as(C.c_void_p), ptr(out), n))
-        return out
-
-    def rvs(self, size=None):
-        arrays, scalars = self._args()
-        n = _common_length(size, *arrays)
-        if size is not None and int(size) != n:        # numpy.random's broadcast error
-            raise ValueError(f"shape mismatch: {n} parameter values cannot be broadcast to size {int(size)}")
-        ctx = context()
-        out = empty(n, dtype=torch.int64 if self.dtype == np.int64 else torch.float64)
-        _lib.check(ctx.lib.smcb_dist_rvs(ctx.handle, self._law, *[ptr(a) for a in arrays],
-                                         scalars.ctypes.data_as(C.c_void_p), ptr(out), n))
-        return out
-
-
 class InvGamma(_KernelLaw):
     """Inverse Gamma(a, b) -- particles/distributions.py:358-377 (scipy.stats.invgamma(a, scale=b)); draws
     b / Gamma(a, 1) from the device Gamma sampler."""

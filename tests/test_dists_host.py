@@ -10,10 +10,12 @@ import mpmath as mp
 import numpy as np
 import pytest
 from scipy import stats
+from scipy.special import gammaln
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BUILD = os.path.join(ROOT, "oracle", "_build")
 INVGAMMA, LOGNORMAL, TRUNCNORMAL, BINOMIAL, GEOMETRIC, NEGBINOMIAL, DUNIFORM, GAMMA = range(8)
+NORMAL, STUDENT, LAPLACE, LOGISTIC = range(8, 12)
 SEED = 20261018
 
 _lib = None
@@ -91,6 +93,37 @@ def test_invgamma_lognormal_logpdf():
     close(host_logpdf(LOGNORMAL, xs, a - 4.0, b), stats.lognorm.logpdf(xs, b, scale=np.exp(a - 4.0)))
     assert np.isnan(host_logpdf(INVGAMMA, [1.0, 1.0], [0.0, 1.0], [1.0, -1.0])).all()
     assert np.isnan(host_logpdf(LOGNORMAL, [1.0], 0.0, 0.0)).all()
+
+
+def student_c0(df):
+    """the host-computed constant of Student's log-density (its lgamma terms)"""
+    return gammaln(0.5 * (df + 1.0)) - gammaln(0.5 * df) - 0.5 * np.log(df * np.pi)
+
+
+def test_normal_student_gamma_laplace_logistic_logpdf():
+    """the laws of state-space models' PX / PY against scipy: NaN, +-inf, 0, negative x (Gamma's xlogy cases at
+    a < 1, a == 1, a > 1), |z| near 700 (Logistic's exp(-|z|) form), scalar and per-element parameters"""
+    x = np.concatenate([[-np.inf, -700.0, -3.0, -0.0, 0.0, 1e-300, np.inf, np.nan, 699.5, 700.5, 710.0],
+                        np.linspace(-8.0, 12.0, 81)])
+    mid = x[~(np.abs(x) > 600.0)]          # scipy's laplace.logpdf is the log of its pdf: -inf once that underflows
+    with np.errstate(all="ignore"):
+        for loc, s in [(0.0, 1.0), (0.5, 2.0), (-3.0, 0.1)]:
+            close(host_logpdf(NORMAL, x, loc, s), stats.norm.logpdf(x, loc, s))
+            close(host_logpdf(LAPLACE, mid, loc, s), stats.laplace.logpdf(mid, loc, s))
+            close(host_logpdf(LOGISTIC, x, loc, s), stats.logistic.logpdf(x, loc, s))
+            for df in (1.0, 2.5, 30.0):
+                close(host_logpdf(STUDENT, x, df, loc, s, student_c0(df)), stats.t.logpdf(x, df, loc, s))
+        for a, b in [(0.4, 2.0), (1.0, 1.0), (1.0, 0.3), (3.5, 2.0), (40.0, 5.0)]:
+            close(host_logpdf(GAMMA, x, a, b, -gammaln(a)), stats.gamma.logpdf(x, a, scale=1.0 / b))
+    r = np.random.RandomState(7)
+    n = 2000
+    xs, loc, s, df = r.normal(0.0, 3.0, n), r.normal(size=n), r.uniform(0.1, 4.0, n), r.uniform(0.5, 50.0, n)
+    close(host_logpdf(NORMAL, xs, loc, s), stats.norm.logpdf(xs, loc, s))
+    close(host_logpdf(STUDENT, xs, df, loc, s, student_c0(df)), stats.t.logpdf(xs, df, loc, s))
+    close(host_logpdf(LAPLACE, xs, loc, s), stats.laplace.logpdf(xs, loc, s))
+    close(host_logpdf(LOGISTIC, xs, loc, s), stats.logistic.logpdf(xs, loc, s))
+    a, b, g = r.uniform(0.2, 9.0, n), r.uniform(0.1, 5.0, n), r.gamma(2.0, 1.0, n)
+    close(host_logpdf(GAMMA, g, a, b, -gammaln(a)), stats.gamma.logpdf(g, a, scale=1.0 / b))
 
 
 def _truncnorm_mp(x, mu, s, a, b):

@@ -7,10 +7,11 @@ import os
 import numpy as np
 import pytest
 from scipy import stats
-from scipy.special import logsumexp
+from scipy.special import gammaln, logsumexp
 
-from test_dists_host import (BINOMIAL, DUNIFORM, GAMMA, GEOMETRIC, INVGAMMA, LOGNORMAL, NEGBINOMIAL, TRUNCNORMAL,
-                             chi2_p, close, host_dirichlet_rvs, host_logpdf, host_rvs, ks_p)
+from test_dists_host import (BINOMIAL, DUNIFORM, GAMMA, GEOMETRIC, INVGAMMA, LAPLACE, LOGISTIC, LOGNORMAL,
+                             NEGBINOMIAL, NORMAL, STUDENT, TRUNCNORMAL, chi2_p, close, host_dirichlet_rvs, host_logpdf,
+                             host_rvs, ks_p, student_c0)
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -51,6 +52,13 @@ def cases(D):
         "Geometric": (lambda *p: D.Geometric(*p), GEOMETRIC, (0.25,), k),
         "NegativeBinomial": (lambda *p: D.NegativeBinomial(*p), NEGBINOMIAL, (3.5, 0.3), k),
         "DiscreteUniform": (lambda *p: D.DiscreteUniform(*p), DUNIFORM, (-1.0, 7.0), k),
+        "Normal": (lambda *p: D.Normal(*p), NORMAL, (0.5, 2.0), x),
+        "Student": (lambda df, loc, s, c0: D.Student(df, loc, s), STUDENT, (2.5, 0.5, 2.0, student_c0(2.5)), x),
+        "GammaSmallA": (lambda a, b, c0: D.Gamma(a, b), GAMMA, (0.4, 2.0, -gammaln(0.4)), x),
+        "GammaExponential": (lambda a, b, c0: D.Gamma(a, b), GAMMA, (1.0, 0.7, -gammaln(1.0)), x),
+        "Gamma": (lambda a, b, c0: D.Gamma(a, b), GAMMA, (3.5, 2.0, -gammaln(3.5)), x),
+        "Laplace": (lambda *p: D.Laplace(*p), LAPLACE, (0.5, 2.0), x),
+        "Logistic": (lambda *p: D.Logistic(*p), LOGISTIC, (0.5, 2.0), x),
     }
 
 
@@ -68,6 +76,10 @@ def test_logpdf_scalar_and_per_particle(D):
             pp[0] = pp[0] + r.normal(size=n)
         elif law in (BINOMIAL, NEGBINOMIAL, GEOMETRIC):
             pp[-1] = r.uniform(0.05, 0.95, n)
+        elif law in (NORMAL, LAPLACE, LOGISTIC):
+            pp = [p * r.uniform(0.5, 1.5, n) for p in pp]
+        elif law in (STUDENT, GAMMA):            # df, a and the constant c0 stay scalars, as in distributions.py
+            pp = [pars[0]] + [p * r.uniform(0.5, 1.5, n) for p in pp[1:-1]] + [pars[-1]]
         xs = r.choice(x[np.isfinite(x)], n)
         got = host(make(*[cuda(p) for p in pp]).logpdf(cuda(xs)))
         close(got, host_logpdf(law, xs, *pp))
@@ -80,6 +92,18 @@ def test_logpdf_scalar_and_per_particle(D):
     ks = np.floor(r.rand(n) * (nn + 1))
     close(host(D.Binomial(cuda(nn), cuda(p)).logpdf(torch.as_tensor(ks, device="cuda").long())),
           stats.binom.logpmf(ks, nn, p))
+
+
+def test_rvs_only_for_laws_with_a_sampler(D):
+    """Normal, Student, Laplace and Logistic draw outside the law table: smcb_dist_rvs refuses their codes"""
+    import ctypes as C
+    from particles_b200 import _lib
+    from particles_b200.device import context, empty, ptr
+    ctx, out, s = context(), empty(8), np.ones(4)
+    for law in (NORMAL, STUDENT, LAPLACE, LOGISTIC):
+        with pytest.raises(ValueError, match="not a law with a sampler"):
+            _lib.check(ctx.lib.smcb_dist_rvs(ctx.handle, law, None, None, None, None, s.ctypes.data_as(C.c_void_p),
+                                             ptr(out), 8))
 
 
 def test_logpdf_against_reference_golden(D, golden):

@@ -69,16 +69,17 @@ def test_weights_scan_search_resample(ctx):
                    "multinomial": 7, "residual": 9, "ssp": 5}
 
 
-def test_distributions(ctx):
+def test_distributions_and_law_table(ctx):
     L = ctx.lib
     x, out = buf(fill=0.25), buf()
     loc0, scale0 = np.zeros(16), np.ones(16)
+    pars = np.array([1.0, 1.0, 1.0, 0.0])        # scalar parameters of law codes 7-11
     got = {
         "uniform": launches(ctx, L.smcb_uniform, p(out), N),
         "standard_normal": launches(ctx, L.smcb_standard_normal, p(out), N),
         "normal_rvs": launches(ctx, L.smcb_normal_rvs, None, 0.0, None, 1.0, None, p(out), N),
-        "normal_logpdf": launches(ctx, L.smcb_normal_logpdf, p(x), 0.0, None, 0.0, None, 1.0, p(out), N),
-        "logpdf1": launches(ctx, L.smcb_logpdf1, 2, p(x), 0.0, 0.0, 0.0, None, 0.0, None, 1.0, p(out), N),
+        **{f"dist_logpdf {law}": launches(ctx, L.smcb_dist_logpdf, law, p(x), 0.0, None, None, None, None, hp(pars),
+                                          p(out), N) for law in range(7, 12)},
         "device_math": launches(ctx, L.smcb_device_math, 0, p(x), p(out), N),
         "device_math table": launches(ctx, L.smcb_device_math, 4, p(x), p(out), N),
     }
